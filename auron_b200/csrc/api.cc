@@ -191,6 +191,17 @@ int auron_b200_tz_offset(const char* zone, int64_t utc_second, int32_t* offset) 
     API_GUARD_END(-1)
 }
 
+int auron_b200_digest_hex(int32_t alg, const uint8_t* bytes, int64_t len, char* out) {
+    API_GUARD_BEGIN
+    AURON_CHECK(out && len >= 0 && (len == 0 || bytes), "null buffer or negative length");
+    if (digest_hex_width(alg) < 0) {
+        g_last_error = "unknown digest algorithm " + std::to_string(alg);
+        return -1;
+    }
+    return digest_hex_host(alg, bytes, len, out);
+    API_GUARD_END(-1)
+}
+
 // ---- device residency
 static std::map<int, std::unique_ptr<Ctx>>& util_ctxs() {
     static std::map<int, std::unique_ptr<Ctx>> m;

@@ -58,6 +58,8 @@ ExprPtr lit_i64(int64_t v);
 ExprPtr lit_null(const DType& t);
 
 DType infer_type(const Expr& e, const Schema& input);
+// the Spark string constructors (concat, concat_ws, repeat, space) and digests (md5, sha2) the projection compiler builds
+bool makes_string_fn(const std::string& name);
 // true when the expression is a bare column reference; *idx receives the resolved index
 bool is_plain_column(const Expr& e, const Schema& input, int* idx);
 

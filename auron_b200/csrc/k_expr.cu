@@ -53,7 +53,11 @@ enum Op : uint16_t {
     OP_MATH1, OP_POW, OP_HASH,
     OP_BITAND, OP_BITOR, OP_BITXOR, OP_SHL, OP_SHR,
     OP_OUT, OP_OUT_PRED, OP_FMT_OUT,
+    OP_SB_BEGIN, OP_SB_APPEND, OP_SB_END,
 };
+// OP_SB_APPEND: flags = piece kind | SB_WS (concat_ws) | SB_REPEAT; aux = output | constant << 8 (the separator with SB_WS, the
+// count with SB_REPEAT); aux2 = FmtKind << 8 | scale of an SB_FMT piece
+enum SbPiece : int { SB_VIEW = 0, SB_FMT = 1, SB_SPACE = 2, SB_WS = 4, SB_REPEAT = 8 };
 enum DatePart : int { DP_YEAR = 0, DP_MONTH, DP_DAY, DP_DOW, DP_QUARTER, DP_WEEK, DP_DOY };
 enum Math1 : int { M_SQRT = 0, M_EXP, M_LN, M_LOG10, M_LOG2, M_SIN, M_COS, M_TAN, M_ASIN, M_ACOS, M_ATAN, M_CEIL, M_FLOOR, M_SIGNUM, M_TRUNC, M_EXPM1 };
 
@@ -706,6 +710,16 @@ __device__ inline int fmt_value(int kind, int scale, uint64_t lo, char* buf) {
     return k;
 }
 
+// copy a string view into an output, applying the ASCII upper (xf 1) / lower (xf 2) mark of OP_CASEXF
+__device__ __forceinline__ void copy_view(uint8_t* d, const uint8_t* s, int32_t len, int xf) {
+    for (int32_t k = 0; k < len; k++) {
+        uint8_t c = s[k];
+        if (xf == 1 && c >= 'a' && c <= 'z') c -= 32;
+        else if (xf == 2 && c >= 'A' && c <= 'Z') c += 32;
+        d[k] = c;
+    }
+}
+
 template <bool HI>
 __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
     extern __shared__ __align__(16) uint64_t vm_smem[];
@@ -713,6 +727,7 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
     int64_t* HIp = (int64_t*)(vm_smem + (HI ? VM_NREG * VM_THREADS : 0));
     Instr* prog = (Instr*)(vm_smem + (HI ? 2 : 1) * VM_NREG * VM_THREADS);
     const int tid = threadIdx.x;
+    char buf[44];   // CAST(x AS STRING) text of OP_FMT_OUT / OP_SB_APPEND
     for (int i = tid; i < p.n_instr * (int)(sizeof(Instr) / 4); i += VM_THREADS) ((uint32_t*)prog)[i] = ((const uint32_t*)p.prog)[i];
     __syncthreads();
 
@@ -1207,16 +1222,7 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                                 if (active) p.out_lens[o][i] = v ? (int64_t)str_len(x) : 0;
                             } else if (v) {
                                 int64_t h = RHI(ins.a);
-                                const uint8_t* s = str_ptr(p, h, x);
-                                uint8_t* d = (uint8_t*)p.out_data[o] + p.out_off[o][i];
-                                int32_t len = str_len(x);
-                                int xf = (int)((h >> 8) & 0xff);
-                                for (int32_t k = 0; k < len; k++) {
-                                    uint8_t c = s[k];
-                                    if (xf == 1 && c >= 'a' && c <= 'z') c -= 32;
-                                    else if (xf == 2 && c >= 'A' && c <= 'Z') c += 32;
-                                    d[k] = c;
-                                }
+                                copy_view((uint8_t*)p.out_data[o] + p.out_off[o][i], str_ptr(p, h, x), str_len(x), (int)((h >> 8) & 0xff));
                             }
                         }
                         if (p.mode == 0) {
@@ -1251,7 +1257,6 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                 case OP_FMT_OUT: {   // CAST(value AS STRING) straight into a utf8 output column (both passes format the value)
                     const int o = ins.aux;
                     bool v = active && VALID(ins.a);
-                    char buf[44];
                     int len = v ? fmt_value((ins.aux2 >> 8) & 0xff, ins.aux2 & 0xff, RLO(ins.a), buf) : 0;
                     if (p.mode == 0) {
                         if (active) p.out_lens[o][i] = len;
@@ -1260,6 +1265,68 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                     } else if (v) {
                         uint8_t* d = (uint8_t*)p.out_data[o] + p.out_off[o][i];
                         for (int k = 0; k < len; k++) d[k] = (uint8_t)buf[k];
+                    }
+                    break;
+                }
+                // String builder (concat / concat_ws / repeat / space) into utf8 output `o`: dst holds the cursor (LO), whether a
+                // piece was emitted (HI) and the row's validity.  Pass 0 adds up the piece lengths, pass 1 copies each piece at
+                // out_off[i] + cursor; it takes the validity pass 0 found, so a row that ends NULL writes nothing.
+                case OP_SB_BEGIN: {
+                    const int o = ins.aux;
+                    RLO(ins.dst) = 0;
+                    if (HI) RHI(ins.dst) = 0;
+                    SETV(ins.dst, active && (p.mode == 0 || ((p.out_valid[o][i >> 5] >> (i & 31)) & 1u)));
+                    break;
+                }
+                case OP_SB_APPEND: {
+                    if (!HI || !VALID(ins.dst)) break;
+                    const int kind = ins.flags & 3;
+                    if (!VALID(ins.a)) {   // concat: a NULL piece makes the row NULL; concat_ws skips it
+                        if (!(ins.flags & SB_WS)) SETV(ins.dst, false);
+                        break;
+                    }
+                    const int o = ins.aux & 0xff;
+                    int64_t cur = (int64_t)RLO(ins.dst);
+                    uint8_t* d = p.mode == 1 ? (uint8_t*)p.out_data[o] + p.out_off[o][i] : nullptr;
+                    if ((ins.flags & SB_WS) && RHI(ins.dst)) {
+                        const uint64_t sep = p.consts[ins.aux >> 8].lo;
+                        if (d) copy_view(d + cur, p.pool + (uint32_t)(sep >> 32), str_len(sep), 0);
+                        cur += str_len(sep);
+                    }
+                    RHI(ins.dst) = 1;
+                    const uint64_t x = RLO(ins.a);
+                    if (kind == SB_SPACE) {
+                        const int64_t n = (int32_t)x > 0 ? (int32_t)x : 0;
+                        if (d)
+                            for (int64_t k = 0; k < n; k++) d[cur + k] = ' ';
+                        cur += n;
+                    } else {   // a view or a formatted value, once or `times` times
+                        const int64_t times = (ins.flags & SB_REPEAT) ? (int64_t)p.consts[ins.aux >> 8].lo : 1;
+                        const uint8_t* s;
+                        int32_t len;
+                        int xf = 0;
+                        if (kind == SB_FMT) {
+                            len = fmt_value((ins.aux2 >> 8) & 0xff, ins.aux2 & 0xff, x, buf);
+                            s = (const uint8_t*)buf;
+                        } else {
+                            const int64_t h = RHI(ins.a);
+                            s = str_ptr(p, h, x);
+                            len = str_len(x);
+                            xf = (int)((h >> 8) & 0xff);
+                        }
+                        for (int64_t r = 0; d && r < times; r++) copy_view(d + cur + r * len, s, len, xf);
+                        cur += times * len;
+                    }
+                    RLO(ins.dst) = (uint64_t)cur;
+                    break;
+                }
+                case OP_SB_END: {
+                    const int o = ins.aux;
+                    const bool v = VALID(ins.a);
+                    if (p.mode == 0) {
+                        if (active) p.out_lens[o][i] = v ? (int64_t)RLO(ins.a) : 0;
+                        uint32_t w = __ballot_sync(FULL_MASK, v);
+                        if ((tid & 31) == 0 && active) p.out_valid[o][i >> 5] = w;
                     }
                     break;
                 }
@@ -1498,6 +1565,13 @@ struct VmProgramImpl {
     std::string pool;
     std::vector<int> in_cols;     // VM input slot -> input schema column index
     std::vector<uint8_t> out_vt;  // VM type per output
+    // md5 / sha2 outputs: hashed after the VM from an input column or from a hidden utf8 output of the program (numbered
+    // after the visible outputs)
+    struct Digest {
+        int out, alg, col, hidden;   // col >= 0: input column, else output `hidden`
+    };
+    std::vector<Digest> digests;
+    int n_hidden = 0;
     bool need_hi = false;
     // device copies (uploaded lazily per ctx stream; programs are immutable after compile)
     Buf d_code, d_consts, d_pool;
@@ -1569,6 +1643,35 @@ bool is_plain_column(const Expr& e, const Schema& input, int* idx) {
     return true;
 }
 
+// Spark string constructors and digests (NativeConverters.scala:927-942,1033-1047): their result is a new utf8 value, which the
+// VM builds only as a whole projection output (OP_SB_*) and digests only after the VM (k_digest.cu)
+static bool is_string_builder(const std::string& f) {
+    return f == "Spark_StringConcat" || f == "Spark_StringConcatWs" || f == "Spark_StringRepeat" || f == "Spark_StringSpace";
+}
+static int digest_alg_of(const std::string& f) {
+    return f == "Spark_MD5" ? DIGEST_MD5 : f == "Spark_Sha224" ? DIGEST_SHA224 : f == "Spark_Sha256" ? DIGEST_SHA256 :
+           f == "Spark_Sha384" ? DIGEST_SHA384 : f == "Spark_Sha512" ? DIGEST_SHA512 : 0;
+}
+bool makes_string_fn(const std::string& f) { return is_string_builder(f) || digest_alg_of(f) != 0; }
+static bool makes_string(const Expr& e) { return e.kind == E_SCALAR_FN && makes_string_fn(e.name); }
+// the planner's declared-type TRY_CAST around one of them (operators.cc ProjectExec) is the identity: their type is utf8
+static const Expr& strip_utf8_cast(const Expr& e) {
+    if ((e.kind == E_CAST || e.kind == E_TRY_CAST) && e.type.id == T_UTF8 && makes_string(*e.children[0])) return *e.children[0];
+    return e;
+}
+// CAST(x AS STRING) of the kinds fmt_value formats (-1: not one of them)
+static int fmt_kind_of(const DType& st, int* scale) {
+    *scale = 0;
+    if (st.id == T_BOOL) return FMT_BOOL;
+    if (st.is_integer()) return FMT_INT;
+    if (st.id == T_DATE32) return FMT_DATE;
+    if (st.id == T_DECIMAL128 && st.precision <= 18 && st.scale >= 0 && st.scale <= 18) {
+        *scale = st.scale;
+        return FMT_DEC;
+    }
+    return -1;
+}
+
 static bool is_cmp_op(const std::string& op) {
     return op == "Eq" || op == "NotEq" || op == "Lt" || op == "LtEq" || op == "Gt" || op == "GtEq" || op == "IsDistinctFrom" || op == "IsNotDistinctFrom";
 }
@@ -1587,6 +1690,7 @@ DType infer_type(const Expr& e, const Schema& in) {
         case E_CASE: return infer_type(*e.children[e.has_case_expr ? 2 : 1], in);
         case E_CAST: case E_TRY_CAST: return e.type;
         case E_SCALAR_FN:
+            if (makes_string(e)) return DType(T_UTF8);
             if (e.type.id != T_NULL) return e.type;
             return infer_type(*e.children[0], in);
     }
@@ -1838,6 +1942,7 @@ struct Compiler {
             emit(OP_TIMEPART, a.reg, a.reg, 0, 0, VT_I32, 0, which);
             return Val{a.reg, DType(T_INT32)};
         };
+        if (makes_string(e)) fail(f + " is only native as a whole projection expression or as the argument of md5 / sha2");
         Val r{-1, DType()};
         if (f == "Spark_Year") r = date_fn(DP_YEAR);
         else if (f == "Spark_Month") r = date_fn(DP_MONTH);
@@ -2096,6 +2201,101 @@ struct Compiler {
         }
         fail("unsupported expression kind");
     }
+
+    // one piece of a string constructor: a utf8 value (view), a formatted CAST to utf8, `times` copies of a view, or spaces
+    void append_piece(const std::string& f, int b, int o, const Expr& x, int flags, int const_idx = 0) {
+        if ((flags & 3) == SB_SPACE) {   // space(n): n is an int32 value, never text
+            const DType nt = infer_type(x, in);
+            if (nt.id != T_INT32 && nt.id != T_NULL) fail(f + " needs an int32 argument, got " + nt.str());
+            Val v = gen(x);
+            if (v.type.id != T_INT32 && v.type.id != T_NULL) fail(f + " needs an int32 argument, got " + v.type.str());
+            emit(OP_SB_APPEND, b, v.reg, 0, 0, VT_I32, flags, o);
+            release(v.reg);
+            return;
+        }
+        int scale = 0, kind = -1;
+        if ((x.kind == E_CAST || x.kind == E_TRY_CAST) && x.type.id == T_UTF8) {
+            const DType st = infer_type(*x.children[0], in);
+            kind = fmt_kind_of(st, &scale);
+            if (kind < 0 && st.id != T_UTF8 && st.id != T_NULL) fail(f + ": CAST " + st.str() + " -> utf8 is not native on device");
+        }
+        Val v = kind >= 0 ? gen(*x.children[0]) : gen(x);
+        if (kind >= 0) {
+            note_type(v.type);
+            emit(OP_SB_APPEND, b, v.reg, 0, 0, vt_of(v.type), SB_FMT | flags, o | (const_idx << 8), (kind << 8) | scale);
+        } else {
+            if (v.type.id != T_UTF8 && v.type.id != T_NULL) fail(f + " argument of type " + v.type.str() + " is not native (utf8 pieces only)");
+            emit(OP_SB_APPEND, b, v.reg, 0, 0, VT_STR, flags, o | (const_idx << 8));
+        }
+        release(v.reg);
+    }
+    // concat (spark_strings.rs:117-192), concat_ws (:194-319), repeat (:75-91), space (:65-73) into utf8 output `o`.  Each piece is
+    // generated, appended and released before the next, so the registers in use do not grow with the number of arguments.
+    void build_string(const Expr& e, int o) {
+        const std::string& f = e.name;
+        const int b = alloc();
+        note_type(DType(T_UTF8));
+        emit(OP_SB_BEGIN, b, 0, 0, 0, VT_STR, 0, o);
+        auto null_row = [&]() {   // a NULL literal argument that makes every row NULL
+            Val v = literal(Literal{DType(T_UTF8), true});
+            emit(OP_SB_APPEND, b, v.reg, 0, 0, VT_STR, SB_VIEW, o);
+            release(v.reg);
+        };
+        auto is_lit = [](const Expr& x) { return x.kind == E_LITERAL; };
+        if (f == "Spark_StringConcat") {
+            for (auto& ch : e.children) append_piece(f, b, o, *ch, SB_VIEW);
+        } else if (f == "Spark_StringConcatWs") {
+            if (e.children.empty() || !is_lit(*e.children[0]) || e.children[0]->lit.type.id != T_UTF8)
+                fail(f + " separator must be a utf8 literal");
+            const Literal& sep = e.children[0]->lit;
+            if (sep.is_null) null_row();
+            else {
+                const int sep_ci = add_pool_string(sep.s);
+                for (size_t k = 1; k < e.children.size(); k++) {
+                    const Expr& x = *e.children[k];
+                    if (is_lit(x) && x.lit.is_null) continue;   // a NULL argument is skipped, separator included
+                    append_piece(f, b, o, x, SB_VIEW | SB_WS, sep_ci);
+                }
+            }
+        } else if (f == "Spark_StringRepeat") {
+            if (e.children.size() != 2 || !is_lit(*e.children[1]) || e.children[1]->lit.type.id != T_INT32)
+                fail(f + " count must be an int32 literal");
+            const Literal& n = e.children[1]->lit;
+            if (n.is_null) null_row();
+            else append_piece(f, b, o, *e.children[0], SB_VIEW | SB_REPEAT, add_const((uint64_t)std::max<int64_t>(0, n.i), 0, true));
+        } else {   // Spark_StringSpace
+            if (e.children.size() != 1) fail(f + " takes one argument");
+            append_piece(f, b, o, *e.children[0], SB_SPACE);
+        }
+        emit(OP_SB_END, 0, b, 0, 0, VT_STR, 0, o);
+        release(b);
+    }
+    // the whole projection expression `ex` into output `o`; returns its type
+    DType output(const Expr& ex, int o) {
+        if (ex.kind == E_SCALAR_FN && is_string_builder(ex.name)) {
+            build_string(ex, o);
+            return DType(T_UTF8);
+        }
+        if ((ex.kind == E_CAST || ex.kind == E_TRY_CAST) && ex.type.id == T_UTF8) {
+            int scale = 0;
+            const int kind = fmt_kind_of(infer_type(*ex.children[0], in), &scale);
+            if (kind >= 0) {   // formatted directly into the output column
+                Val v = gen(*ex.children[0]);
+                note_type(v.type);
+                note_type(ex.type);
+                emit(OP_FMT_OUT, 0, v.reg, 0, 0, vt_of(v.type), 0, o, (kind << 8) | scale);
+                release(v.reg);
+                return ex.type;
+            }
+        }
+        Val v = gen(ex);
+        DType t = v.type;
+        if (t.id == T_NULL) fail("projection of an untyped NULL");
+        note_type(t);
+        emit(OP_OUT, 0, v.reg, 0, 0, vt_of(t), 0, o);
+        release(v.reg);
+        return t;
+    }
 };
 
 VmProgram compile_projection(const std::vector<ExprPtr>& exprs, const Schema& input) {
@@ -2104,31 +2304,26 @@ VmProgram compile_projection(const std::vector<ExprPtr>& exprs, const Schema& in
     Compiler c(input, *p.impl);
     AURON_CHECK(exprs.size() <= VM_MAX_COLS, "too many projection expressions for one program");
     for (size_t i = 0; i < exprs.size(); i++) {
-        const Expr& ex = *exprs[i];
-        if ((ex.kind == E_CAST || ex.kind == E_TRY_CAST) && ex.type.id == T_UTF8) {
-            DType st = infer_type(*ex.children[0], input);
-            int kind = -1, scale = 0;
-            if (st.id == T_BOOL) kind = FMT_BOOL;
-            else if (st.is_integer()) kind = FMT_INT;
-            else if (st.id == T_DATE32) kind = FMT_DATE;
-            else if (st.id == T_DECIMAL128 && st.precision <= 18 && st.scale >= 0 && st.scale <= 18) kind = FMT_DEC, scale = st.scale;
-            if (kind >= 0) {   // formatted directly into the output column; a string CAST nested inside another expression is not built
-                Compiler::Val v = c.gen(*ex.children[0]);
-                c.note_type(v.type);
-                c.note_type(ex.type);
-                c.emit(OP_FMT_OUT, 0, v.reg, 0, 0, vt_of(v.type), 0, (int)i, (kind << 8) | scale);
-                c.release(v.reg);
-                p.out_types.push_back(ex.type);
-                p.impl->out_vt.push_back(VT_STR);
-                continue;
+        const Expr& ex = strip_utf8_cast(*exprs[i]);
+        const int alg = ex.kind == E_SCALAR_FN ? digest_alg_of(ex.name) : 0;
+        if (alg) {   // spark_crypto.rs:33-105: the digest of a utf8 or binary value's bytes
+            if (ex.children.size() != 1) fail(ex.name + " takes one argument");
+            const Expr& arg = strip_utf8_cast(*ex.children[0]);
+            const DType at = infer_type(arg, input);
+            if (!at.is_varlen()) fail(ex.name + " needs a utf8 or binary argument, got " + at.str());
+            VmProgramImpl::Digest d{(int)i, alg, -1, -1};
+            if (!is_plain_column(arg, input, &d.col)) {
+                d.col = -1;
+                d.hidden = (int)exprs.size() + p.impl->n_hidden++;
+                AURON_CHECK(d.hidden < VM_MAX_COLS, "too many projection expressions for one program");
+                c.output(arg, d.hidden);
             }
+            p.impl->digests.push_back(d);
+            p.out_types.push_back(DType(T_UTF8));
+            p.impl->out_vt.push_back(VT_STR);
+            continue;
         }
-        Compiler::Val v = c.gen(*exprs[i]);
-        DType t = v.type;
-        if (t.id == T_NULL) fail("projection of an untyped NULL");
-        c.note_type(t);
-        c.emit(OP_OUT, 0, v.reg, 0, 0, vt_of(t), 0, (int)i);
-        c.release(v.reg);
+        const DType t = c.output(ex, (int)i);
         p.out_types.push_back(t);
         p.impl->out_vt.push_back(vt_of(t));
     }
@@ -2294,14 +2489,29 @@ __global__ void narrow_offsets_kernel2(const int64_t* __restrict__ off64, int32_
     if (i < n_plus_1) off32[i] = (int32_t)off64[i];
 }
 
+// utf8 output `c` from its int64 row lengths: offsets by an exclusive scan, then the data buffer
+static void finish_offsets(Ctx& ctx, Column& c, int64_t* lens, int64_t n) {
+    exclusive_scan_i64(ctx, lens, lens, n, lens + n);
+    narrow_offsets_kernel2<<<(unsigned)((n + 1 + 255) / 256), 256, 0, ctx.stream>>>(lens, P<int32_t>(c.offsets), n + 1);
+    LAUNCH_CHECK(ctx);
+    int64_t total = 0;
+    to_host(ctx, &total, lens + n, 8);
+    AURON_CHECK(total <= (int64_t)INT32_MAX, "utf8 column exceeds 2 GiB in one batch");
+    c.data = dalloc(ctx, (size_t)total);
+    c.data_bytes = total;
+}
+
 std::vector<ColumnPtr> eval_projection(Ctx& ctx, const VmProgram& prog, const Batch& in, const int32_t* sel, int64_t n_out) {
     init_pow10_tables();
     VmProgramImpl& im = *prog.impl;
+    const size_t n_vis = prog.out_types.size(), n_all = n_vis + (size_t)im.n_hidden;   // hidden outputs: digest arguments
+    std::vector<bool> digested(n_all, false);
+    for (auto& d : im.digests) digested[(size_t)d.out] = true;
     std::vector<ColumnPtr> outs;
-    std::vector<Buf> lens(prog.out_types.size());
-    bool any_str = false;
-    for (size_t i = 0; i < prog.out_types.size(); i++) {
-        const DType& t = prog.out_types[i];
+    std::vector<Buf> lens(n_all);
+    bool vm_str = false;
+    for (size_t i = 0; i < n_all; i++) {
+        const DType t = i < n_vis ? prog.out_types[i] : DType(T_UTF8);
         auto c = std::make_shared<Column>();
         c->type = t;
         c->len = n_out;
@@ -2311,7 +2521,7 @@ std::vector<ColumnPtr> eval_projection(Ctx& ctx, const VmProgram& prog, const Ba
         else if (t.is_varlen()) {
             lens[i] = dalloc(ctx, (size_t)(n_out + 1) * 8);
             c->offsets = dalloc(ctx, (size_t)(n_out + 1) * 4);
-            any_str = true;
+            vm_str = vm_str || !digested[i];
         } else c->data = dalloc(ctx, (size_t)n_out * t.width());
         outs.push_back(c);
     }
@@ -2321,37 +2531,42 @@ std::vector<ColumnPtr> eval_projection(Ctx& ctx, const VmProgram& prog, const Ba
                 CUDA_OK(cudaMemsetAsync(c->offsets->ptr, 0, 4, ctx.stream));
                 c->data = dalloc(ctx, 0);
             }
+        outs.resize(n_vis);
         return outs;
     }
-    upload(ctx, im);
-    VmParams p;
-    bind_inputs(im, in, p);
-    p.sel = sel;
-    p.n = n_out;
-    p.mode = 0;
-    for (size_t i = 0; i < outs.size(); i++) {
-        p.out_data[i] = outs[i]->data ? outs[i]->data->ptr : nullptr;
-        p.out_valid[i] = P<uint32_t>(outs[i]->validity);
-        p.out_lens[i] = P<int64_t>(lens[i]);
-    }
-    launch_vm(ctx, im, p);
-    if (any_str) {
+    if (!im.code.empty()) {
+        upload(ctx, im);
+        VmParams p;
+        bind_inputs(im, in, p);
+        p.sel = sel;
+        p.n = n_out;
+        p.mode = 0;
         for (size_t i = 0; i < outs.size(); i++) {
-            if (!outs[i]->type.is_varlen()) continue;
-            exclusive_scan_i64(ctx, P<int64_t>(lens[i]), P<int64_t>(lens[i]), n_out, P<int64_t>(lens[i]) + n_out);
-            narrow_offsets_kernel2<<<(unsigned)((n_out + 1 + 255) / 256), 256, 0, ctx.stream>>>(P<int64_t>(lens[i]), P<int32_t>(outs[i]->offsets), n_out + 1);
-            LAUNCH_CHECK(ctx);
-            int64_t total = 0;
-            to_host(ctx, &total, P<int64_t>(lens[i]) + n_out, 8);
-            AURON_CHECK(total <= (int64_t)INT32_MAX, "utf8 column exceeds 2 GiB in one batch");
-            outs[i]->data = dalloc(ctx, (size_t)total);
-            outs[i]->data_bytes = total;
-            p.out_data[i] = outs[i]->data->ptr;
-            p.out_off[i] = P<int32_t>(outs[i]->offsets);
+            p.out_data[i] = outs[i]->data ? outs[i]->data->ptr : nullptr;
+            p.out_valid[i] = P<uint32_t>(outs[i]->validity);
+            p.out_lens[i] = P<int64_t>(lens[i]);
         }
-        p.mode = 1;
         launch_vm(ctx, im, p);
+        if (vm_str) {
+            for (size_t i = 0; i < outs.size(); i++) {
+                if (!outs[i]->type.is_varlen() || digested[i]) continue;
+                finish_offsets(ctx, *outs[i], P<int64_t>(lens[i]), n_out);
+                p.out_data[i] = outs[i]->data->ptr;
+                p.out_off[i] = P<int32_t>(outs[i]->offsets);
+            }
+            p.mode = 1;
+            launch_vm(ctx, im, p);
+        }
     }
+    for (auto& d : im.digests) {   // k_digest.cu: one launch per digest output, after the VM built any argument it needed
+        const Column& src = d.col >= 0 ? *in.cols[(size_t)d.col] : *outs[(size_t)d.hidden];
+        const int32_t* s = d.col >= 0 ? sel : nullptr;
+        Column& out = *outs[(size_t)d.out];
+        digest_lengths(ctx, src.vbits(), s, n_out, d.alg, P<uint32_t>(out.validity), P<int64_t>(lens[(size_t)d.out]));
+        finish_offsets(ctx, out, P<int64_t>(lens[(size_t)d.out]), n_out);
+        digest_hex(ctx, d.alg, P<int32_t>(src.offsets), P<uint8_t>(src.data), s, n_out, P<int32_t>(out.offsets), P<uint8_t>(out.data));
+    }
+    outs.resize(n_vis);
     return outs;
 }
 

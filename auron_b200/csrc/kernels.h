@@ -37,6 +37,18 @@ Buf murmur3_partition_ids(Ctx& ctx, const std::vector<ColumnPtr>& cols, int64_t 
 Buf bound_ranks(Ctx& ctx, const int32_t* perm, int64_t n, int64_t nb);   // range partitioning (k_sort.cu)
 Buf round_robin_partition_ids(Ctx& ctx, int64_t n, int64_t start, int32_t num_parts);   // (i + start) % num_parts
 
+// ----------------------------------------------------------------------------- k_digest.cu
+// Spark md5 / sha2 as lowercase hex (spark_crypto.rs:33-105); the algorithm is named by its digest length in bits
+enum DigestAlg : int { DIGEST_MD5 = 128, DIGEST_SHA224 = 224, DIGEST_SHA256 = 256, DIGEST_SHA384 = 384, DIGEST_SHA512 = 512 };
+int digest_hex_width(int alg);   // 32 / 56 / 64 / 96 / 128 characters, -1 for an unknown algorithm
+// lens[i] = hex width when row sel[i] (sel == nullptr: row i) of in_valid is valid, else 0; out_valid = that validity
+void digest_lengths(Ctx& ctx, const uint8_t* in_valid, const int32_t* sel, int64_t n, int alg, uint32_t* out_valid, int64_t* lens);
+// hex digests of the utf8 / binary rows sel[i] into out at out_off[i]; an empty output range marks a NULL row
+void digest_hex(Ctx& ctx, int alg, const int32_t* in_off, const uint8_t* in_data, const int32_t* sel, int64_t n, const int32_t* out_off,
+                uint8_t* out);
+// the same computation on the CPU: writes digest_hex_width(alg) characters to out, returns that width or -1
+int digest_hex_host(int alg, const uint8_t* bytes, int64_t len, char* out);
+
 // ----------------------------------------------------------------------------- k_rowkeys.cu
 // Row-key view over key columns for hash aggregation / joins (general path)
 struct KeyColDesc {

@@ -536,8 +536,14 @@ ExprPtr decode_expr(const uint8_t* b, size_t n) {
                 while (s.next(&sf, &sw)) {
                     if (sf == 1 && sw == 2) nm = s.bytes();
                     else if (sf == 2 && sw == 0) fun = (int)s.varint();
-                    else if (sf == 3 && sw == 2) e->children.push_back(child(s));
-                    else if (sf == 4 && sw == 2) {
+                    else if (sf == 3 && sw == 2) {
+                        try {
+                            e->children.push_back(child(s));
+                        } catch (const Error& err) {   // e.g. an array<string> argument of concat_ws: say which function it was
+                            if (makes_string_fn(nm)) fail(nm + ": " + err.what());
+                            throw;
+                        }
+                    } else if (sf == 4 && sw == 2) {
                         const uint8_t* tb;
                         size_t tn;
                         s.bytes_view(&tb, &tn);

@@ -153,6 +153,11 @@ int64_t auron_b200_explain(const uint8_t* task_definition, size_t len, char* out
  * date/time functions that take a session time zone (spark_dates.rs:93-110,200-227, chrono-tz in the reference).
  * Returns 0 and fills *offset, or -1 when `zone` is not an IANA zone name.  Host only: usable without a GPU. */
 int auron_b200_tz_offset(const char* zone, int64_t utc_second, int32_t* offset);
+/* Lowercase hex digest of `len` bytes, computed by the same compression and padding code the device's md5 / sha2 kernels run
+ * (Spark_MD5, Spark_Sha224/256/384/512, spark_crypto.rs:33-105).  `alg` is the digest length in bits: 128 (MD5), 224, 256, 384
+ * or 512.  Writes 32 / 56 / 64 / 96 / 128 characters to `out` (no terminator) and returns that count, or -1 for an unknown `alg`.
+ * Host only: usable without a GPU. */
+int auron_b200_digest_hex(int32_t alg, const uint8_t* bytes, int64_t len, char* out);
 /* What the engine's Parquet metadata reader sees in the local file `path`, as JSON: footer (schema elements, row groups, column
  * chunks with codec / sizes / offsets / statistics as hex) plus, per chunk, the walk of its page headers (page counts, value
  * counts, encodings; SNAPPY bodies are run through the engine's block decoder).  The reference reads the same structures with

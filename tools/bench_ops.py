@@ -2,12 +2,18 @@
 time per launch site from the library's CUDA-event timers (AURON_PROFILE=1).  These are the operator-level numbers the
 north star asks for next to the config-2 bench line; they are not bench.py lines.
 
-    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard]
+    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project]
 
   join     cfg 3: store_sales (N rows: ss_sold_date_sk int32, ss_item_sk int32, ss_quantity int32) JOIN date_dim (73,049 rows:
            d_date_sk int32, d_year int32) on the date key, inner, build = date_dim
   sort     cfg 4 (one GPU's share): ORDER BY ss_item_sk over (ss_item_sk int32, ss_ticket_number int64, ss_ext_sales_price decimal(7,2))
   shuffle  cfg 4: hash repartition of the same rows on ss_item_sk into 200 partitions, compacted shuffle format to /dev/shm
+  strings  md5(s), sha2(s, 256), sha2(s, 512), concat_ws('|', cast(i as string), s) and md5(concat_ws(...)) over N rows of
+           (s utf8, i int64), once with a mean string length of ~32 B and once with ~200 B; each projection feeds a COUNT so that
+           one row leaves the GPU.  Reports compression-function calls per second next to rows/s and input GB/s.
+  filter_project  cfg 1 shape on the expression VM: Project[a + 1, substr(s, 1, 4), CAST(d * 3 AS decimal(38, 2))] <-
+           Filter[a > 100000 AND s LIKE 'a%'] over N rows (a int64 1 % NULL, s utf8 4-24 B, d int64), + COUNT / SUM so that one
+           row leaves the GPU; the decimal output runs the 128-bit variant of vm_kernel
 """
 import os
 import sys
@@ -66,6 +72,7 @@ def run(plan, label, rows, steps=4, alg=None):
     for _, op, name, v in m:
         if op != "__kernels__" and name.endswith("_ns") and v > 2e5:
             print(f"     [{op}.{name} = {v / 1e6:.2f} ms]")
+    return kern
 
 
 if "join" in which:
@@ -144,3 +151,78 @@ if "sort" in which or "shuffle" in which:
             if op != "__kernels__" and name.endswith("_ns") and v > 2e5:
                 print(f"     [{op}.{name} = {v / 1e6:.2f} ms]")
     runtime.drop_device_resource("t4")
+
+if "strings" in which:
+    import subprocess
+
+    def text_len(x):   # characters of CAST(int64 AS STRING)
+        a = np.abs(x)
+        return (x < 0).astype(np.int64) + 1 + sum((a >= 10 ** k).astype(np.int64) for k in range(1, 19))
+
+    def digest_calls(lens, block, pad):   # compression-function calls: floor((len + pad) / block) + 1 per row
+        return int(((lens + pad) // block + 1).sum())
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"== strings leg on: {gpu}")
+    for mean in (32, 200):
+        chunk = min(CHUNK, (1 << 31) // (2 * mean + 160))   # keeps every utf8 input and output of one batch below 2 GiB
+        pool = rng.integers(32, 127, 1 << 20, dtype=np.uint8)
+        lens_all, ws_all = [], []
+        for start in range(0, N, chunk):
+            n = min(chunk, N - start)
+            lens = rng.integers(0, 2 * mean + 1, n).astype(np.int64)
+            offs = np.zeros(n + 1, dtype=np.int32)
+            np.cumsum(lens, out=offs[1:])
+            data = np.resize(pool, int(offs[-1]))
+            s_arr = pa.Array.from_buffers(pa.string(), n, [None, pa.py_buffer(offs), pa.py_buffer(data)])
+            i_np = rng.integers(-2**62, 2**62, n, dtype=np.int64)
+            runtime.put_device_batch(f"str{mean}", pa.record_batch([s_arr, pa.array(i_np)], names=["s", "i"]))
+            lens_all.append(lens)
+            ws_all.append(lens + 1 + text_len(i_np))
+        lens = np.concatenate(lens_all)
+        ws_lens = np.concatenate(ws_all)
+        s_in = int(lens.sum()) + 4 * (N + 1)            # algorithmic bytes: string bytes + offsets
+        ws_out = int(ws_lens.sum()) + 4 * (N + 1)
+        schema = pa.schema([("s", pa.string()), ("i", pa.int64())])
+        U = pa.string()
+        ws = P.scalar_fn("Spark_StringConcatWs", [P.lit("|", U), P.cast(P.col("i"), U), P.col("s")], U)
+        hexb = lambda w: N * w + 4 * (N + 1)   # noqa: E731
+        # label, expression, {launch site: algorithmic bytes}, (digest site, compression calls)
+        cases = [("md5(s)", P.scalar_fn("Spark_MD5", [P.col("s")], U), {"digest_md5": s_in + hexb(32)}, ("digest_md5", digest_calls(lens, 64, 8))),
+                 ("sha2(s,256)", P.scalar_fn("Spark_Sha256", [P.col("s")], U), {"digest_sha256": s_in + hexb(64)},
+                  ("digest_sha256", digest_calls(lens, 64, 8))),
+                 ("sha2(s,512)", P.scalar_fn("Spark_Sha512", [P.col("s")], U), {"digest_sha512": s_in + hexb(128)},
+                  ("digest_sha512", digest_calls(lens, 128, 16))),
+                 ("concat_ws('|', cast(i as string), s)", ws, {"expr_vm": s_in + 8 * N + ws_out}, None),
+                 ("md5(concat_ws(...))", P.scalar_fn("Spark_MD5", [ws], U), {"expr_vm": s_in + 8 * N + ws_out, "digest_md5": ws_out + hexb(32)},
+                  ("digest_md5", digest_calls(ws_lens, 64, 8)))]
+        for label, expr, alg, digest in cases:
+            proj = P.projection(P.ffi_reader(schema, f"str{mean}"), [expr], ["h"], [U])
+            plan = P.agg(proj, [], [], [P.agg_expr("COUNT", [P.col("h")], pa.int64())], ["c"], ["PARTIAL"])
+            us = run(plan, f"strings mean {mean} B: {label} over {N} rows", N, steps=3, alg=alg)
+            if digest and us.get(digest[0]):
+                site, calls = digest
+                t = us[site] * 1e-6
+                print(f"     {site}: {N / t / 1e9:.2f} G rows/s, {alg[site] / t / 1e9:.0f} GB/s algorithmic, "
+                      f"{calls / t / 1e9:.2f} G compression calls/s ({calls / N:.2f} per row)")
+        runtime.drop_device_resource(f"str{mean}")
+
+if "filter_project" in which:
+    pool = rng.integers(97, 123, 1 << 20, dtype=np.uint8)
+    for start in range(0, N, CHUNK):
+        n = min(CHUNK, N - start)
+        lens = rng.integers(4, 25, n)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        np.cumsum(lens, out=offs[1:])
+        s_arr = pa.Array.from_buffers(pa.string(), n, [None, pa.py_buffer(offs), pa.py_buffer(np.resize(pool, int(offs[-1])))])
+        a = pa.array(rng.integers(0, 1_000_000, n), type=pa.int64(), mask=rng.random(n) < 0.01)
+        runtime.put_device_batch("fp", pa.record_batch([a, s_arr, pa.array(rng.integers(-10**9, 10**9, n), type=pa.int64())], names=["a", "s", "d"]))
+    sch = pa.schema([("a", pa.int64()), ("s", pa.string()), ("d", pa.int64())])
+    flt = P.filter_(P.ffi_reader(sch, "fp"), [P.binary("Gt", P.col("a"), P.lit(100000, pa.int64())), P.like(P.col("s"), P.lit("a%", pa.string()))])
+    proj = P.projection(flt, [P.binary("Plus", P.col("a"), P.lit(1, pa.int64())),
+                              P.scalar_fn("Substr", [P.col("s"), P.lit(1, pa.int64()), P.lit(4, pa.int64())], pa.string()),
+                              P.cast(P.binary("Multiply", P.col("d"), P.lit(3, pa.int64())), pa.decimal128(38, 2))],
+                        ["a1", "s4", "dd"], [pa.int64(), pa.string(), pa.decimal128(38, 2)])
+    plan = P.agg(proj, [], [], [P.agg_expr("COUNT", [P.col("s4")], pa.int64()), P.agg_expr("SUM", [P.col("a1")], pa.int64())], ["c", "x"], ["PARTIAL"] * 2)
+    run(plan, f"cfg1 shape Filter -> Project (decimal output) over {N} rows", N, steps=6)
+    runtime.drop_device_resource("fp")
