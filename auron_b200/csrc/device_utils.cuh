@@ -12,6 +12,16 @@ namespace auron {
 __device__ __forceinline__ bool bit_get(const uint8_t* bm, int64_t i) { return (bm[i >> 3] >> (i & 7)) & 1; }
 __device__ __forceinline__ bool valid_at(const uint8_t* bm, int64_t i) { return bm == nullptr || bit_get(bm, i); }
 __device__ __forceinline__ unsigned lane_id() { return threadIdx.x & 31; }
+// byte-wise (unsigned, shorter-prefix-first) order of two rows of a utf8 / binary column: < 0, 0, > 0
+__device__ __forceinline__ int str_row_cmp(const uint8_t* __restrict__ data, const int32_t* __restrict__ offs, int64_t a, int64_t b) {
+    const int32_t a0 = offs[a], la = offs[a + 1] - a0, b0 = offs[b], lb = offs[b + 1] - b0;
+    const int32_t m = la < lb ? la : lb;
+    for (int32_t i = 0; i < m; i++) {
+        const int d = (int)data[a0 + i] - (int)data[b0 + i];
+        if (d) return d;
+    }
+    return la - lb;
+}
 __device__ __forceinline__ unsigned lanemask_lt() {
     unsigned m;
     asm("mov.u32 %0, %%lanemask_lt;" : "=r"(m));

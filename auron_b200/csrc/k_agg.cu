@@ -130,17 +130,6 @@ __device__ __forceinline__ bool acc_load(const AccDesc& d, int64_t row, int64_t 
     }
     return false;
 }
-// byte-wise (unsigned, shorter-prefix-first) order of two rows of a utf8 / binary column: < 0, 0, > 0
-__device__ __forceinline__ int str_row_cmp(const uint8_t* __restrict__ data, const int32_t* __restrict__ offs, int64_t a, int64_t b) {
-    const int32_t a0 = offs[a], la = offs[a + 1] - a0, b0 = offs[b], lb = offs[b + 1] - b0;
-    const int32_t m = la < lb ? la : lb;
-    for (int32_t i = 0; i < m; i++) {
-        const int d = (int)data[a0 + i] - (int)data[b0 + i];
-        if (d) return d;
-    }
-    return la - lb;
-}
-
 // STR: the kernel instance handles string extremes (MIN_STR / MAX_STR).  Compiled into every instance, the CAS loop below
 // slows the SUM / COUNT path of agg_direct_kernel, so plans without string extremes
 // run instances that do not contain it.

@@ -140,13 +140,26 @@ JoinPairs join_probe(Ctx& ctx, const JoinTable& t, const std::vector<ColumnPtr>&
                      uint32_t* matched_build, Buf* probe_matched_out);
 
 // ----------------------------------------------------------------------------- k_window.cu
-// rows sorted by (partition keys, order keys): flags[i] = 1 where row i starts a new group of `keys` (row 0 always; `also`: boundaries to inherit)
-Buf window_boundaries(Ctx& ctx, const std::vector<ColumnPtr>& keys, int64_t n, const uint8_t* also);
-ColumnPtr window_rank_column(Ctx& ctx, int func /* 0 ROW_NUMBER, 1 RANK, 2 DENSE_RANK */, const uint8_t* pflags, const uint8_t* oflags, int64_t n);
-ColumnPtr window_agg_column(Ctx& ctx, int fn /* AggFunction: 0 MIN, 1 MAX, 2 SUM, 3 AVG, 4 COUNT */, const ColumnPtr& arg, const DType& out_type, const uint8_t* pflags, int64_t n);
+// rows sorted by (partition keys, order keys): flags[i] = 1 where row i starts a new group of `keys` (`also`: boundaries to inherit).
+// prev: the keys of the previous batch's last row (one row per column; empty without keys) -- row 0 starts a group where they differ;
+// nullptr: there is no previous row, row 0 starts a group.
+Buf window_boundaries(Ctx& ctx, const std::vector<ColumnPtr>& keys, int64_t n, const uint8_t* also, const std::vector<ColumnPtr>* prev);
+// the last row that starts a new group of `keys`, -1 when none does; row 0 counts only when prev (the keys of the row before it, one
+// row per column) is given and differs.  Synchronises.
+int64_t window_last_boundary(Ctx& ctx, const std::vector<ColumnPtr>& keys, int64_t n, const std::vector<ColumnPtr>* prev);
+// the state of a running window function at the last row computed so far, carried into the next batch (empty: nothing before it)
+struct WinCarry {
+    Buf a, b;          // scan values at that row (see the functions below)
+    ColumnPtr value;   // one-row column that owns its bytes (string MIN / MAX, NTH_VALUE)
+};
+// carry (optional): read when set, then replaced by the state at row n - 1
+ColumnPtr window_rank_column(Ctx& ctx, int func /* 0 ROW_NUMBER, 1 RANK, 2 DENSE_RANK */, const uint8_t* pflags, const uint8_t* oflags, int64_t n, WinCarry* carry);
+ColumnPtr window_agg_column(Ctx& ctx, int fn /* AggFunction: 0 MIN, 1 MAX, 2 SUM, 3 AVG, 4 COUNT */, const ColumnPtr& arg, const DType& out_type, const uint8_t* pflags, int64_t n,
+                            WinCarry* carry);
+ColumnPtr window_nth_column(Ctx& ctx, const ColumnPtr& values, int64_t nth, bool ignore_nulls, const uint8_t* pflags, int64_t n, WinCarry* carry);
+// these look at the whole partition: the rows passed in hold complete partitions
 ColumnPtr window_dist_column(Ctx& ctx, int func /* 6 PERCENT_RANK, 7 CUME_DIST */, const uint8_t* pflags, const uint8_t* oflags, int64_t n);
 ColumnPtr window_lead_column(Ctx& ctx, const ColumnPtr& values, const ColumnPtr& defaults, int64_t offset, const uint8_t* pflags, int64_t n);
-ColumnPtr window_nth_column(Ctx& ctx, const ColumnPtr& values, int64_t nth, bool ignore_nulls, const uint8_t* pflags, int64_t n);
 Buf window_le_mask(Ctx& ctx, const ColumnPtr& rank_col, int32_t k);   // bit mask of rows with rank <= k (WindowGroupLimit)
 
 // ----------------------------------------------------------------------------- k_sort.cu

@@ -1086,15 +1086,38 @@ WindowExec::WindowExec(OperatorPtr input, std::vector<ExprPtr> part, std::vector
     if (output_window_cols)
         for (auto& f : funcs) out_schema.fields.push_back(f.field);
     AURON_CHECK(group_limit < 0 || funcs.size() == 1, "WindowGroupLimit expects exactly one rank-like window function (window_exec.rs:341-344)");
+    static const char* af[] = {"MIN", "MAX", "SUM", "AVG", "COUNT"};
+    const Schema& is = input->out_schema;
     for (auto& f : funcs) {
-        if (f.is_agg) AURON_CHECK(f.func >= 0 && f.func <= 4, "window aggregate function #" + std::to_string(f.func) + " is not native in auron_b200 (MIN / MAX / SUM / AVG / COUNT are)");
-        else {
+        if (f.is_agg) {
+            AURON_CHECK(f.func >= 0 && f.func <= 4, "window aggregate function #" + std::to_string(f.func) + " is not native in auron_b200 (MIN / MAX / SUM / AVG / COUNT are)");
+            if (f.args.empty()) {   // COUNT(*)-like: every row counts
+                AURON_CHECK(f.func == AGG_COUNT, std::string("window ") + af[f.func] + " without an argument");
+                continue;
+            }
+            // the argument types of agg/{sum,avg,maxmin,count}.rs, checked when the plan is built
+            const DType at = infer_type(*f.args[0], is);
+            bool ok = true;
+            if (f.func == AGG_SUM || f.func == AGG_AVG) ok = at.is_integer() || at.id == T_DATE32 || at.is_float() || at.id == T_DECIMAL128;
+            else if (f.func == AGG_MIN || f.func == AGG_MAX) ok = at.is_intlike() || at.is_float() || at.id == T_DECIMAL128 || at.is_varlen() || at.id == T_BOOL;
+            AURON_CHECK(ok, std::string("window ") + af[f.func] + " over " + at.str() + " is not supported");
+            // SUM / AVG with a decimal result: TryCast(arg, return type) first, as AggExec does (agg.rs:191-198)
+            if ((f.func == AGG_SUM || f.func == AGG_AVG) && f.field.type.id == T_DECIMAL128 && !load_compatible(at, f.field.type)) {
+                auto c = std::make_shared<Expr>();
+                c->kind = E_TRY_CAST;
+                c->type = f.field.type;
+                c->children.push_back(f.args[0]);
+                f.args[0] = c;
+            }
+        } else {
             AURON_CHECK(f.func >= 0 && f.func <= 7, "window function #" + std::to_string(f.func) + " is not native in auron_b200");
             auto int_literal = [&](size_t i) { return f.args.size() > i && f.args[i]->kind == E_LITERAL && !f.args[i]->lit.is_null && f.args[i]->lit.type.width() > 0 && f.args[i]->lit.type.width() <= 8; };
             if (f.func == 3) AURON_CHECK(f.args.size() == 3 && int_literal(1), "LEAD expects input / literal integer offset / default children (lead_processor.rs:40-63)");
             if (f.func == 4 || f.func == 5) AURON_CHECK(f.args.size() == 2 && int_literal(1) && f.args[1]->lit.i > 0, "NTH_VALUE expects input / positive literal offset children (nth_value_processor.rs:36-66)");
+            whole_partition = whole_partition || f.func == 3 || f.func == 6 || f.func == 7;   // window/mod.rs:115-120
         }
     }
+    carries.resize(funcs.size());
     children.push_back(std::move(input));
 }
 std::string WindowExec::describe() const {
@@ -1108,32 +1131,98 @@ std::string WindowExec::describe() const {
     for (size_t i = 0; i < funcs.size(); i++) o += (i ? "," : "") + json_quote(std::string(funcs[i].is_agg ? af[funcs[i].func] : wf[funcs[i].func]) + " AS " + funcs[i].field.name);
     return o + "],\"group_limit\":" + std::to_string(group_limit) + ",\"output_window_cols\":" + (output_window_cols ? "true" : "false");
 }
-BatchPtr WindowExec::next(Task& t) {
-    if (done) return nullptr;
-    done = true;
-    // every function is a scan over the complete sorted input (the reference streams partition by partition; here the whole input
-    // of the task is one device batch, like the sort below it that produced the order)
-    std::vector<BatchPtr> all;
-    while (BatchPtr b = children[0]->next(t)) {
-        AURON_CHECK(t.is_running(), "task killed");
-        if (b->num_rows) all.push_back(b);
+// rows [0, len) of a batch without a copy: the columns share the buffers (an Arrow array may have longer buffers than it uses)
+static BatchPtr prefix_view(Task& t, const Batch& in, int64_t len) {
+    auto out = std::make_shared<Batch>();
+    out->num_rows = len;
+    for (auto& c : in.cols) {
+        auto v = std::make_shared<Column>(*c);
+        v->len = len;
+        if (c->null_count == c->len) v->null_count = len;
+        else if (c->null_count != 0) v->null_count = -1;
+        if (c->type.is_varlen()) {
+            int32_t end = 0;
+            to_host(t.ctx, &end, P<int32_t>(c->offsets) + len, 4);
+            v->data_bytes = end;
+        }
+        out->cols.push_back(v);
     }
-    if (all.empty()) return nullptr;
-    BatchPtr in = all.size() == 1 ? all[0] : concat_batches(t.ctx, all);
-    all.clear();
+    return out;
+}
+BatchPtr WindowExec::take_staged(Task& t, const BatchPtr& extra) {
+    std::vector<BatchPtr> parts;
+    parts.swap(staged);
+    staged_last.clear();
+    if (extra) parts.push_back(extra);
+    AURON_CHECK(!parts.empty(), "WindowExec: no rows held back");   // cut == 0 is only found against a held-back row
+    if (parts.size() == 1) return parts[0];
+    int64_t rows = 0;
+    for (auto& b : parts) rows += b->num_rows;
+    metrics.add("concat_rows", rows);
+    return concat_batches(t.ctx, parts);
+}
+BatchPtr WindowExec::next(Task& t) {
+    while (!done) {
+        BatchPtr in = children[0]->next(t);
+        AURON_CHECK(t.is_running(), "task killed");
+        if (!in) {   // end of input: the rows held back form complete partitions
+            done = true;
+            if (staged.empty()) return nullptr;
+            in = take_staged(t, nullptr);
+        } else {
+            if (in->num_rows == 0) continue;
+            if (whole_partition) {
+                // compute up to the last partition boundary and hold back the open partition (window_exec.rs:227-291); the held-back
+                // batches are kept as they are and concatenated once, when their partition closes; without a partition spec all rows
+                // are held back until the input ends
+                if (partition_exprs.empty()) {
+                    staged.push_back(in);
+                    continue;
+                }
+                const int64_t n = in->num_rows;
+                int64_t cut;
+                std::vector<ColumnPtr> pk;
+                {
+                    OpTimer timer(metrics, "elapsed_ns");
+                    for (auto& e : partition_exprs) pk.push_back(eval_to_column(t, e, children[0]->out_schema, *in));
+                    // the last partition start in this batch; row 0 counts when it differs from the last held-back row
+                    cut = window_last_boundary(t.ctx, pk, n, staged.empty() ? nullptr : &staged_last);
+                }
+                std::vector<ColumnPtr> last;
+                for (auto& c : pk) last.push_back(slice_column(t.ctx, *c, n - 1, 1));
+                if (cut < 0) {   // no partition closes here
+                    staged.push_back(in);
+                    staged_last = std::move(last);
+                    continue;
+                }
+                // the held-back rows and rows [0, cut) form complete partitions; rows [cut, n) are the open one
+                const BatchPtr batch = in;
+                in = take_staged(t, cut > 0 ? prefix_view(t, *batch, cut) : nullptr);
+                staged.push_back(cut > 0 ? slice_batch(t.ctx, *batch, cut, n - cut) : batch);
+                staged_last = std::move(last);
+            }
+        }
+        if (BatchPtr out = compute(t, in)) return out;
+    }
+    return nullptr;
+}
+BatchPtr WindowExec::compute(Task& t, const BatchPtr& in) {
     OpTimer timer(metrics, "elapsed_ns");
     const int64_t n = in->num_rows;
     const Schema& is = children[0]->out_schema;
     std::vector<ColumnPtr> pk, ok;
     for (auto& e : partition_exprs) pk.push_back(eval_to_column(t, e, is, *in));
     for (auto& e : order_exprs) ok.push_back(eval_to_column(t, e, is, *in));
-    Buf pflags = window_boundaries(t.ctx, pk, n, nullptr);
-    Buf oflags = window_boundaries(t.ctx, ok, n, P<uint8_t>(pflags));   // a new partition starts a new peer group
+    // row 0 continues the previous batch's partition (peer group) when its keys equal those of that batch's last row
+    Buf pflags = window_boundaries(t.ctx, pk, n, nullptr, has_prev ? &prev_part : nullptr);
+    Buf oflags = window_boundaries(t.ctx, ok, n, P<uint8_t>(pflags), has_prev ? &prev_order : nullptr);   // a new partition starts a new peer group
     std::vector<ColumnPtr> wcols;
-    for (auto& f : funcs) {
+    for (size_t i = 0; i < funcs.size(); i++) {
+        const WindowFuncSpec& f = funcs[i];
+        WinCarry* carry = &carries[i];
         if (!f.is_agg && f.func <= 2) {
             AURON_CHECK(f.field.type.id == T_INT32, "rank-like window functions return int32");
-            wcols.push_back(window_rank_column(t.ctx, f.func, P<uint8_t>(pflags), P<uint8_t>(oflags), n));
+            wcols.push_back(window_rank_column(t.ctx, f.func, P<uint8_t>(pflags), P<uint8_t>(oflags), n, carry));
         } else if (!f.is_agg && (f.func == 6 || f.func == 7)) {
             AURON_CHECK(f.field.type.id == T_FLOAT64, "PERCENT_RANK / CUME_DIST return float64");
             wcols.push_back(window_dist_column(t.ctx, f.func, P<uint8_t>(pflags), P<uint8_t>(oflags), n));
@@ -1144,22 +1233,25 @@ BatchPtr WindowExec::next(Task& t) {
             wcols.push_back(window_lead_column(t.ctx, vals, dflt, f.args[1]->lit.i, P<uint8_t>(pflags), n));
         } else if (!f.is_agg) {                  // NTH_VALUE [IGNORE NULLS](input, n)
             ColumnPtr vals = eval_to_column(t, f.args[0], is, *in);
-            wcols.push_back(window_nth_column(t.ctx, vals, f.args[1]->lit.i, f.func == 5, P<uint8_t>(pflags), n));
+            wcols.push_back(window_nth_column(t.ctx, vals, f.args[1]->lit.i, f.func == 5, P<uint8_t>(pflags), n, carry));
         } else {
             ColumnPtr arg;
-            if (f.args.empty()) {   // COUNT(*)-like: every row counts
-                AURON_CHECK(f.func == 4, "window aggregate without an argument");
-                arg = make_column(t.ctx, DType(T_INT8), n, false);
-            } else arg = eval_to_column(t, f.args[0], is, *in);
-            wcols.push_back(window_agg_column(t.ctx, f.func, arg, f.field.type, P<uint8_t>(pflags), n));
+            if (f.args.empty()) arg = make_column(t.ctx, DType(T_INT8), n, false);   // COUNT(*)-like: every row counts
+            else arg = eval_to_column(t, f.args[0], is, *in);
+            wcols.push_back(window_agg_column(t.ctx, f.func, arg, f.field.type, P<uint8_t>(pflags), n, carry));
         }
     }
+    prev_part.clear();
+    prev_order.clear();
+    for (auto& c : pk) prev_part.push_back(slice_column(t.ctx, *c, n - 1, 1));
+    for (auto& c : ok) prev_order.push_back(slice_column(t.ctx, *c, n - 1, 1));
+    has_prev = true;
     auto out = std::make_shared<Batch>();
     out->num_rows = n;
     out->cols = in->cols;
     if (output_window_cols)
         for (auto& c : wcols) out->cols.push_back(c);
-    if (group_limit >= 0) {   // keep the rows whose rank is <= k (window_exec.rs:341-356)
+    if (group_limit >= 0) {   // keep the rows whose rank is <= k (window_exec.rs:341-356); the rank carries across batches
         Buf mask = window_le_mask(t.ctx, wcols[0], (int32_t)std::min<int64_t>(group_limit, INT32_MAX));
         int64_t cnt = 0;
         Buf idx = mask_to_indices(t.ctx, P<uint32_t>(mask), n, &cnt);

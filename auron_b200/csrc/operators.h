@@ -166,10 +166,13 @@ struct HashJoinExec : Operator {
 };
 
 // window_exec.rs:162-345 + window/processors/*.rs.  The input arrives sorted by (partition spec, order spec); every window function is a
-// segmented scan (+ one scatter / gather for the functions that look at the whole partition) over the whole input (k_window.cu).
+// segmented scan (+ one scatter / gather for the functions that look at the whole partition) over one input batch (k_window.cu).
 // Built: ROW_NUMBER, RANK, DENSE_RANK, PERCENT_RANK, CUME_DIST, LEAD, NTH_VALUE [IGNORE NULLS], running SUM / COUNT / MIN / MAX / AVG
-// over integers, dates and floats, WindowGroupLimit (keep the rows with rank <= k) and output_window_cols = false.  Not built:
-// aggregates over decimals / strings (rejected by name).
+// (SUM / AVG over integers, dates, floats and decimals; MIN / MAX also over strings, binary, booleans, date64 and timestamps),
+// WindowGroupLimit (keep the rows with rank <= k) and output_window_cols = false.
+// Batches stream through (window_exec.rs:224-304): the running functions carry their state at the last row into the next batch.
+// When a function needs the whole partition (PERCENT_RANK, CUME_DIST, LEAD), the open partition at the end of a batch is held back
+// and concatenated once with the rows that close it; without a partition spec that holds back the whole input.
 struct WindowFuncSpec {
     bool is_agg = false;
     int func = 0;                 // WindowFunction (auron.proto:128-137) or AggFunction (MIN 0, MAX 1, SUM 2, AVG 3, COUNT 4)
@@ -181,9 +184,19 @@ struct WindowExec : Operator {
     std::vector<WindowFuncSpec> funcs;
     int64_t group_limit = -1;
     bool output_window_cols = true, done = false;
+    bool whole_partition = false;                // some function needs the whole partition
+    std::vector<WinCarry> carries;               // per function
+    bool has_prev = false;                       // a batch has been computed: prev_* hold the keys of its last row
+    std::vector<ColumnPtr> prev_part, prev_order;
+    std::vector<BatchPtr> staged;                // rows held back (whole_partition): the open partition, or all rows without a partition spec
+    std::vector<ColumnPtr> staged_last;          // partition keys of the last held-back row (one row each)
     WindowExec(OperatorPtr input, std::vector<ExprPtr> part, std::vector<ExprPtr> order, std::vector<WindowFuncSpec> fs, int64_t limit, bool out_cols);
     std::string describe() const override;
     BatchPtr next(Task& t) override;
+
+   private:
+    BatchPtr compute(Task& t, const BatchPtr& in);   // the window columns of the next rows; nullptr when the group limit keeps none
+    BatchPtr take_staged(Task& t, const BatchPtr& extra);   // the held-back rows (+ extra) as one batch, concatenated once
 };
 
 // sort_merge_join_exec.rs:135-205,294-372 + joins/smj/*.rs.  Both inputs arrive sorted on the join keys.  The reference advances two

@@ -57,6 +57,8 @@ DType decode_arrow_type(const uint8_t* b, size_t n) {
                 break;
             }
             case 3: case 5: case 7: case 9: fail("unsigned integer columns are not supported on device");
+            case 25: case 26: case 27: fail("unsupported ArrowType list (tag " + std::to_string(f) + "): nested types are out of scope");
+            case 28: case 33: fail(std::string("unsupported ArrowType ") + (f == 28 ? "struct" : "map") + " (tag " + std::to_string(f) + "): nested types are out of scope");
             default: fail("unsupported ArrowType tag " + std::to_string(f) + " (nested / interval types are out of scope)");
         }
         (void)v;
@@ -1004,28 +1006,36 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     uint32_t wf, ww;
                     WindowFuncSpec spec;
                     int func_type = 0, window_func = 0, agg_func = 0;
-                    bool have_type = false;
+                    const uint8_t *field_b = nullptr, *type_b = nullptr;
+                    size_t field_n = 0, type_n = 0;
+                    std::vector<std::pair<const uint8_t*, size_t>> arg_b;
                     while (w.next(&wf, &ww)) {
                         const uint8_t* vb;
                         size_t vn;
-                        if (wf == 1 && ww == 2) {
-                            w.bytes_view(&vb, &vn);
-                            spec.field = decode_field(vb, vn);
-                        } else if (wf == 1000 && ww == 2) {
-                            w.bytes_view(&vb, &vn);
-                            spec.field.type = decode_arrow_type(vb, vn);
-                            have_type = true;
-                        } else if (wf == 2 && ww == 0) func_type = (int)w.varint();
+                        if (wf == 1 && ww == 2) w.bytes_view(&field_b, &field_n);
+                        else if (wf == 1000 && ww == 2) w.bytes_view(&type_b, &type_n);
+                        else if (wf == 2 && ww == 0) func_type = (int)w.varint();
                         else if (wf == 3 && ww == 0) window_func = (int)w.varint();
                         else if (wf == 4 && ww == 0) agg_func = (int)w.varint();
                         else if (wf == 5 && ww == 2) {
                             w.bytes_view(&vb, &vn);
-                            spec.args.push_back(decode_expr(vb, vn));
+                            arg_b.emplace_back(vb, vn);
                         } else w.skip(ww);
                     }
-                    (void)have_type;   // return_type repeats the field's type
                     spec.is_agg = func_type == 1;
                     spec.func = spec.is_agg ? agg_func : window_func;
+                    // types and arguments are decoded once the function is known, so that an unsupported one names it
+                    try {
+                        if (field_b) spec.field = decode_field(field_b, field_n);
+                        if (type_b) spec.field.type = decode_arrow_type(type_b, type_n);   // return_type repeats the field's type
+                        for (auto& a : arg_b) spec.args.push_back(decode_expr(a.first, a.second));
+                    } catch (const Error& e) {
+                        static const char* wfn[] = {"ROW_NUMBER", "RANK", "DENSE_RANK", "LEAD", "NTH_VALUE", "NTH_VALUE_IGNORE_NULLS", "PERCENT_RANK", "CUME_DIST"};
+                        static const char* afn[] = {"MIN", "MAX", "SUM", "AVG", "COUNT"};
+                        const int nf = spec.is_agg ? 5 : 8;
+                        const std::string fname = spec.func >= 0 && spec.func < nf ? (spec.is_agg ? afn : wfn)[spec.func] : "#" + std::to_string(spec.func);
+                        fail("window " + fname + ": " + e.what());
+                    }
                     funcs.push_back(std::move(spec));
                 }
                 out.reset(new WindowExec(std::move(input), std::move(part), std::move(order), std::move(funcs), limit, out_cols));

@@ -2,7 +2,7 @@
 time per launch site from the library's CUDA-event timers (AURON_PROFILE=1).  These are the operator-level numbers the
 north star asks for next to the config-2 bench line; they are not bench.py lines.
 
-    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project]
+    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [window]
 
   join     cfg 3: store_sales (N rows: ss_sold_date_sk int32, ss_item_sk int32, ss_quantity int32) JOIN date_dim (73,049 rows:
            d_date_sk int32, d_year int32) on the date key, inner, build = date_dim
@@ -14,6 +14,9 @@ north star asks for next to the config-2 bench line; they are not bench.py lines
   filter_project  cfg 1 shape on the expression VM: Project[a + 1, substr(s, 1, 4), CAST(d * 3 AS decimal(38, 2))] <-
            Filter[a > 100000 AND s LIKE 'a%'] over N rows (a int64 1 % NULL, s utf8 4-24 B, d int64), + COUNT / SUM so that one
            row leaves the GPU; the decimal output runs the 128-bit variant of vm_kernel
+  window   WindowExec over N pre-sorted rows (p int32, ~1,000 rows per partition; o int64; v decimal(17,2), 5 % NULL; s utf8 8-24 B)
+           in device batches of 16M rows, so the running state carries across batch edges: ROW_NUMBER, RANK, SUM(v), AVG(v), MAX(s),
+           COUNT(v) partitioned by p ordered by o, + COUNT / SUM so that one row leaves the GPU
 """
 import os
 import sys
@@ -226,3 +229,44 @@ if "filter_project" in which:
     plan = P.agg(proj, [], [], [P.agg_expr("COUNT", [P.col("s4")], pa.int64()), P.agg_expr("SUM", [P.col("a1")], pa.int64())], ["c", "x"], ["PARTIAL"] * 2)
     run(plan, f"cfg1 shape Filter -> Project (decimal output) over {N} rows", N, steps=6)
     runtime.drop_device_resource("fp")
+
+if "window" in which:
+    import subprocess
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"== window leg on: {gpu}")
+    assert N % 1000 == 0
+    pool = rng.integers(97, 123, 1 << 20, dtype=np.uint8)
+    s_bytes = 0
+    for start in range(0, N, CHUNK):
+        n = min(CHUNK, N - start)
+        p = (np.arange(start, start + n) // 1000).astype(np.int32)
+        o = np.sort(rng.integers(0, 1000, n).reshape(-1, 1000), axis=1).reshape(-1)   # sorted inside every partition of 1,000 rows
+        unscaled = rng.integers(-10**12, 10**12, n)
+        buf = np.empty(2 * n, dtype=np.int64)
+        buf[0::2] = unscaled
+        buf[1::2] = np.where(unscaled < 0, -1, 0)
+        valid = rng.random(n) >= 0.05
+        v = pa.Array.from_buffers(pa.decimal128(17, 2), n, [pa.py_buffer(np.packbits(valid, bitorder="little").tobytes()), pa.py_buffer(buf.tobytes())])
+        lens = rng.integers(8, 25, n)
+        offs = np.zeros(n + 1, dtype=np.int32)
+        np.cumsum(lens, out=offs[1:])
+        s_arr = pa.Array.from_buffers(pa.string(), n, [None, pa.py_buffer(offs), pa.py_buffer(np.resize(pool, int(offs[-1])))])
+        s_bytes += int(offs[-1])
+        runtime.put_device_batch("win", pa.record_batch([pa.array(p), pa.array(o), v, s_arr], names=["p", "o", "v", "s"]))
+    sch = pa.schema([("p", pa.int32()), ("o", pa.int64()), ("v", pa.decimal128(17, 2)), ("s", pa.string())])
+    I, L = pa.int32(), pa.int64()
+    wex = [P.window_expr("rn", I, "ROW_NUMBER"), P.window_expr("rk", I, "RANK"), P.window_expr("sv", pa.decimal128(27, 2), "SUM", [P.col("v")]),
+           P.window_expr("av", pa.decimal128(21, 6), "AVG", [P.col("v")]), P.window_expr("ms", pa.string(), "MAX", [P.col("s")]),
+           P.window_expr("cv", L, "COUNT", [P.col("v")])]
+    win = P.window(P.ffi_reader(sch, "win"), wex, [P.col("p")], [P.sort_expr(P.col("o"))])
+    plan = P.agg(win, [], [], [P.agg_expr("COUNT", [P.col("ms")], L), P.agg_expr("SUM", [P.col("rn")], L), P.agg_expr("SUM", [P.col("rk")], L),
+                               P.agg_expr("COUNT", [P.col("sv")], L), P.agg_expr("COUNT", [P.col("av")], L), P.agg_expr("SUM", [P.col("cv")], L)],
+                 ["c", "rn", "rk", "sv", "av", "cv"], ["PARTIAL"] * 6)
+    # algorithmic bytes per row of the segmented scans (input + output once, + the 1-byte boundary flags): four int64 scans (ROW_NUMBER,
+    # RANK's row number, the COUNT and the two counts of SUM / AVG share the shape) + RANK's max, two i128 value scans, one int32 index
+    # scan for MAX(s); the string gather reads and writes the bytes and offsets once
+    scan_b = N * (17 * 6 + 33 * 2 + 9)
+    run(plan, f"window ROW_NUMBER, RANK, SUM(dec), AVG(dec), MAX(utf8), COUNT over {N} rows in {(N + CHUNK - 1) // CHUNK} batches", N, steps=3,
+        alg={"window_scan": scan_b, "take": 2 * (s_bytes + 4 * N)})
+    runtime.drop_device_resource("win")
