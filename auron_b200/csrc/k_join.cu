@@ -298,7 +298,7 @@ __global__ void __launch_bounds__(256) jkey_minmax(JKey key, int64_t n, long lon
 }
 __global__ void __launch_bounds__(256) jdirect_fill(JKey key, int64_t n, long long dmin, int32_t* __restrict__ direct) {
     const int64_t row = (int64_t)blockIdx.x * 256 + threadIdx.x;
-    if (row < n && !(key.validity && !bit_get(key.validity, row))) direct[(long long)jload_key64(key, row) - dmin] = (int32_t)row;
+    if (row < n && !(key.validity && !bit_get(key.validity, row))) direct[jload_key64(key, row) - (unsigned long long)dmin] = (int32_t)row;
 }
 // (grid-stride: a block counts its matches in registers and adds them once -- one atomic per warp on a single address
 // serialised in L2 and cost 10x the lookups)
@@ -309,7 +309,7 @@ __global__ void __launch_bounds__(256) jprobe_unique_direct(JKey key, const int3
     for (int64_t row = (int64_t)blockIdx.x * 256 + threadIdx.x; row < n32; row += (int64_t)gridDim.x * 256) {
         int32_t b = -1;
         if (row < n && !(key.validity && !bit_get(key.validity, row))) {
-            const unsigned long long d = (unsigned long long)((long long)jload_key64(key, row) - dmin);
+            const unsigned long long d = jload_key64(key, row) - (unsigned long long)dmin;   // wraps for keys below dmin
             if (d <= (unsigned long long)drange) b = __ldg(direct + d);
         }
         if (row < n) build_idx[row] = b;
@@ -402,9 +402,12 @@ std::shared_ptr<JoinTable> join_build(Ctx& ctx, const std::vector<ColumnPtr>& bu
         LAUNCH_CHECK(ctx);
         long long h[2];
         to_host(ctx, h, mm->ptr, 16);
-        if (h[0] <= h[1] && (unsigned long long)(h[1] - h[0]) < (16ull << 20)) {
+        // the span in unsigned arithmetic: h[1] - h[0] overflows int64 when the keys reach both ends of the range, and a compiler
+        // may then fold the signed difference into a small one
+        const unsigned long long span = (unsigned long long)h[1] - (unsigned long long)h[0];
+        if (h[0] <= h[1] && span < (16ull << 20)) {
             t->dmin = h[0];
-            t->drange = (int64_t)(h[1] - h[0]);
+            t->drange = (int64_t)span;
             t->direct = dalloc_fill(ctx, (size_t)(t->drange + 1) * 4, 0xff);
             jdirect_fill<<<blocks, 256, 0, ctx.stream>>>(jk, n_build, t->dmin, P<int32_t>(t->direct));
             LAUNCH_CHECK(ctx);

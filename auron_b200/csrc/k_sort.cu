@@ -363,8 +363,10 @@ bool sort_key_words(Ctx& ctx, const std::vector<SortKeySpec>& keys, int64_t n, s
     }
     return true;
 }
+// the word arrays of a run as a device array of pointers: a key of k columns has up to 3 k words (NULL rank + two decimal128
+// words), so there is no fixed bound to put in a kernel argument
 struct WordPtrs {
-    const uint64_t* w[16];
+    const uint64_t* const* w;
     int nw;
 };
 // out[s * W + w] = word w of row floor((2 s + 1) n / (2 S)): S evenly spaced samples of a sorted run
@@ -394,18 +396,18 @@ __global__ void lower_bound_words_kernel(WordPtrs wp, int64_t n, const uint64_t*
     }
     out[s] = lo;
 }
-static WordPtrs word_ptrs(const std::vector<Buf>& words) {
-    AURON_CHECK(words.size() <= 16, "too many sort key words");
-    WordPtrs wp;
-    wp.nw = (int)words.size();
-    for (int i = 0; i < wp.nw; i++) wp.w[i] = P<uint64_t>(words[(size_t)i]);
-    return wp;
+// *ptrs keeps the pointer array alive until the caller's kernel has been enqueued (frees are stream-ordered)
+static WordPtrs word_ptrs(Ctx& ctx, const std::vector<Buf>& words, Buf* ptrs) {
+    std::vector<const uint64_t*> host(words.size());
+    for (size_t i = 0; i < words.size(); i++) host[i] = P<uint64_t>(words[i]);
+    *ptrs = to_device(ctx, host.data(), host.size() * sizeof(host[0]));
+    return WordPtrs{P<const uint64_t*>(*ptrs), (int)words.size()};
 }
 std::vector<uint64_t> sample_sorted_words(Ctx& ctx, const std::vector<Buf>& words, int64_t n, int S) {
     std::vector<uint64_t> host((size_t)S * words.size());
     if (S <= 0 || n <= 0 || words.empty()) return host;
-    Buf out = dalloc(ctx, host.size() * 8);
-    sample_words_kernel<<<(S + 127) / 128, 128, 0, ctx.stream>>>(word_ptrs(words), n, S, P<uint64_t>(out));
+    Buf out = dalloc(ctx, host.size() * 8), ptrs;
+    sample_words_kernel<<<(S + 127) / 128, 128, 0, ctx.stream>>>(word_ptrs(ctx, words, &ptrs), n, S, P<uint64_t>(out));
     LAUNCH_CHECK(ctx);
     to_host(ctx, host.data(), out->ptr, host.size() * 8);
     return host;
@@ -415,8 +417,8 @@ std::vector<int64_t> lower_bound_sorted_words(Ctx& ctx, const std::vector<Buf>& 
     if (S <= 0) return host;
     if (n <= 0 || words.empty()) return host;
     Buf ds = to_device(ctx, splitters.data(), splitters.size() * 8);
-    Buf out = dalloc(ctx, (size_t)S * 8);
-    lower_bound_words_kernel<<<(S + 127) / 128, 128, 0, ctx.stream>>>(word_ptrs(words), n, P<uint64_t>(ds), S, P<int64_t>(out));
+    Buf out = dalloc(ctx, (size_t)S * 8), ptrs;
+    lower_bound_words_kernel<<<(S + 127) / 128, 128, 0, ctx.stream>>>(word_ptrs(ctx, words, &ptrs), n, P<uint64_t>(ds), S, P<int64_t>(out));
     LAUNCH_CHECK(ctx);
     to_host(ctx, host.data(), out->ptr, (size_t)S * 8);
     return host;
