@@ -14,6 +14,7 @@
 //   * predicate NULL => row dropped (cached_exprs_evaluator.rs:514-519)
 //   * integer + - * wrap (arrow *_wrapping); x / 0 and x % 0 => NULL (Spark_NullIfZero wraps divisors,
 //     datafusion-ext-functions/src/spark_null_if.rs:69-110); Kleene AND/OR
+//   * decimal + - * => NULL when the result leaves i128 or the declared precision of the node (Spark's non-ANSI arithmetic)
 //   * comparisons of floats use IEEE totalOrder like arrow-ord cmp (NaN == NaN, -0 < +0)
 //   * CAST per datafusion-ext-commons/src/arrow/cast.rs: float->int saturating with NaN->0 (:54-95),
 //     utf8->int / utf8->date Spark parsers (:394-529), other numeric casts as arrow safe casts
@@ -143,9 +144,8 @@ __device__ inline i128 u128_divmod(i128 n, i128 d, i128* rem) {
     *rem = r;
     return q;
 }
-// |a| * 10^k with overflow detection (result must stay < 2^127)
-__device__ inline bool u128_mul_pow10(i128 a, int k, i128* out) {
-    i128 m = pow10_128(k);
+// a * m of two magnitudes (< 2^127) with overflow detection (result must stay < 2^127)
+__device__ inline bool u128_mul_checked(i128 a, i128 m, i128* out) {
     // a = a1:a0, m = m1:m0 ; overflow unless a1*m1 == 0 and cross terms fit
     uint64_t a0 = a.lo, a1 = (uint64_t)a.hi, m0 = m.lo, m1 = (uint64_t)m.hi;
     if (a1 != 0 && m1 != 0) return false;
@@ -161,14 +161,40 @@ __device__ inline bool u128_mul_pow10(i128 a, int k, i128* out) {
     *out = {lo, (int64_t)h3};
     return true;
 }
+// |a| * 10^k with overflow detection (result must stay < 2^127)
+__device__ __forceinline__ bool u128_mul_pow10(i128 a, int k, i128* out) { return u128_mul_checked(a, pow10_128(k), out); }
 __device__ __forceinline__ bool dec_fits_precision(i128 v, int prec) {
     if (prec >= 39) return true;
     return u128_lt(i128_abs(v), pow10_128(prec));
 }
+// decimal + - * of unscaled values: false when the exact result leaves i128 or `prec` digits (Spark's non-ANSI arithmetic
+// gives NULL there; a wrapped i128 would be a plausible wrong number)
+__device__ inline bool dec_arith(int op, i128 x, i128 y, int prec, i128* z) {
+    if (op == OP_MUL) {
+        const bool neg = i128_is_neg(x) != i128_is_neg(y);
+        i128 m;
+        if (!u128_mul_checked(i128_abs(x), i128_abs(y), &m)) return false;   // |x|, |y| < 10^38 < 2^127
+        *z = neg ? i128_neg(m) : m;
+    } else {
+        if (op == OP_SUB) y = i128_neg(y);
+        *z = i128_add(x, y);
+        if (((x.hi ^ z->hi) & (y.hi ^ z->hi)) < 0) return false;   // both operands' sign differs from the sum's: wrapped
+    }
+    return dec_fits_precision(*z, prec);
+}
+// correctly rounded (one rounding): the top 64 significant bits with a sticky bit for everything below, then an exact scaling
 __device__ __forceinline__ double i128_to_f64(i128 v) {
     bool neg = i128_is_neg(v);
     i128 a = neg ? i128_neg(v) : v;
-    double d = (double)(uint64_t)a.hi * 18446744073709551616.0 + (double)a.lo;
+    const uint64_t hi = (uint64_t)a.hi;
+    double d;
+    if (hi == 0) d = (double)a.lo;
+    else {
+        const int sh = 64 - __clzll((long long)hi);   // 1..64 bits of `hi` are significant
+        const uint64_t top = sh == 64 ? hi : (hi << (64 - sh)) | (a.lo >> sh);
+        const uint64_t below = sh == 64 ? a.lo : a.lo << (64 - sh);
+        d = ldexp((double)(top | (below != 0)), sh);
+    }
     return neg ? -d : d;
 }
 __device__ inline bool f64_to_i128(double x, i128* out) {
@@ -673,7 +699,7 @@ __device__ inline int fmt_value(int kind, int scale, uint64_t lo, char* buf) {
         if (y < 0) {
             buf[k++] = '-';
             y = -y;
-        }
+        } else if (y > 9999) buf[k++] = '+';   // chrono: years outside 0..9999 as {:+05}
         int yd = fmt_u64((uint64_t)y, end);
         for (int i = yd; i < 4; i++) buf[k++] = '0';
         for (int i = 0; i < yd; i++) buf[k++] = (end - yd)[i];
@@ -826,14 +852,10 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                             case OP_MOD: z = fmod(x, y); break;
                         }
                         r = (uint64_t)__double_as_longlong(z);
-                    } else if (t == VT_DEC && HI) {
+                    } else if (t == VT_DEC && HI) {   // aux: the declared precision of the result
                         i128 x = {a, RHI(ins.a)}, y = {b, RHI(ins.b)}, z = {0, 0};
-                        switch (ins.op) {
-                            case OP_ADD: z = i128_add(x, y); break;
-                            case OP_SUB: z = i128_sub(x, y); break;
-                            case OP_MUL: z = i128_mul(x, y); break;
-                            default: v = false;
-                        }
+                        if (v && !dec_arith(ins.op, x, y, ins.aux, &z)) v = false;
+                        if (!v) z = {0, 0};
                         r = z.lo;
                         RHI(ins.dst) = z.hi;
                     }
@@ -1675,14 +1697,37 @@ static int fmt_kind_of(const DType& st, int* scale) {
 static bool is_cmp_op(const std::string& op) {
     return op == "Eq" || op == "NotEq" || op == "Lt" || op == "LtEq" || op == "Gt" || op == "GtEq" || op == "IsDistinctFrom" || op == "IsNotDistinctFrom";
 }
+// the common type both operands of a decimal comparison, sum or difference are rescaled to (the kernels work on unscaled values)
+static DType dec_common_type(const DType& a, const DType& b) {
+    const int sc = std::max(a.scale, b.scale);
+    const int ip = std::max(a.precision - a.scale, b.precision - b.scale);
+    return DType::decimal(std::min(38, ip + sc), sc);
+}
+// decimal result types as arrow declares them, capped at 38 digits: p1 + p2 + 1 digits at scale s1 + s2 for a product,
+// max(p) + 1 digits at the common scale for a sum or difference; the kernel gives NULL for a result that does not fit
+static DType dec_arith_type(const std::string& op, DType a, DType b) {
+    if (op == "Multiply") return DType::decimal(std::min(38, a.precision + b.precision + 1), a.scale + b.scale);
+    if (a.scale != b.scale) {
+        const DType common = dec_common_type(a, b);
+        if (a.scale != common.scale) a = common;
+        if (b.scale != common.scale) b = common;
+    }
+    return DType::decimal(std::min(38, std::max(a.precision, b.precision) + 1), a.scale);
+}
 
 DType infer_type(const Expr& e, const Schema& in) {
     switch (e.kind) {
         case E_COLUMN: return in.fields[resolve_col(e, in)].type;
         case E_LITERAL: return e.lit.type;
-        case E_BINARY:
+        case E_BINARY: {
             if (is_cmp_op(e.op) || e.op == "And" || e.op == "Or") return DType(T_BOOL);
-            return infer_type(*e.children[0], in);
+            const DType a = infer_type(*e.children[0], in);
+            if (a.id == T_DECIMAL128 && (e.op == "Plus" || e.op == "Minus" || e.op == "Multiply")) {
+                const DType b = infer_type(*e.children[1], in);
+                if (b.id == T_DECIMAL128) return dec_arith_type(e.op, a, b);
+            }
+            return a;
+        }
         case E_NOT: case E_IS_NULL: case E_IS_NOT_NULL: case E_IN_LIST: case E_LIKE: case E_STARTS_WITH: case E_ENDS_WITH: case E_CONTAINS:
         case E_SC_AND: case E_SC_OR:
             return DType(T_BOOL);
@@ -1817,12 +1862,11 @@ struct Compiler {
             } else if (a.type.id == T_DECIMAL128 && b.type.id == T_DECIMAL128) {
                 // the kernels compare / add the unscaled i128 values: both operands must carry the same scale (arrow-rs rescales,
                 // Spark inserts the casts itself; 1.00@2 vs 1.0000@4 must not compare 100 with 10000)
-                if (a.type.scale != b.type.scale) {
-                    const int sc = std::max(a.type.scale, b.type.scale);
-                    const int ip = std::max(a.type.precision - a.type.scale, b.type.precision - b.type.scale);
-                    const DType common = DType::decimal(std::min(38, ip + sc), sc);
-                    if (a.type.scale != sc) a = cast_to(a, common);
-                    if (b.type.scale != sc) b = cast_to(b, common);
+                // (a product needs no common scale: its unscaled value is the product of the operands' at scale s1 + s2)
+                if (a.type.scale != b.type.scale && op != "Multiply") {
+                    const DType common = dec_common_type(a.type, b.type);
+                    if (a.type.scale != common.scale) a = cast_to(a, common);
+                    if (b.type.scale != common.scale) b = cast_to(b, common);
                 }
             } else if (a.type.id == T_TIMESTAMP && b.type.id == T_TIMESTAMP) {
                 AURON_CHECK(a.type.unit == b.type.unit, "binary operator " + op + " on timestamps of different units");
@@ -1858,9 +1902,8 @@ struct Compiler {
         if (t == VT_STR || t == VT_BOOL) fail("arithmetic on " + a.type.str());
         if (t == VT_DEC && (o == OP_DIV || o == OP_MOD || o > OP_MOD))
             fail("decimal " + op + " is not native (auron.decimal.arithOp.enabled=false in the reference)");
-        DType rt = a.type;
-        if (t == VT_DEC && o == OP_MUL) rt = DType::decimal(std::min(38, a.type.precision + b.type.precision + 1), a.type.scale + b.type.scale);
-        emit(o, a.reg, a.reg, b.reg, 0, t);
+        const DType rt = t == VT_DEC ? dec_arith_type(op, a.type, b.type) : a.type;
+        emit(o, a.reg, a.reg, b.reg, 0, t, 0, t == VT_DEC ? rt.precision : 0);
         release(b.reg);
         return {a.reg, rt};
     }
@@ -2375,6 +2418,8 @@ static bool try_compile_simple(const std::vector<ExprPtr>& conjuncts, const Sche
         const DType& ct = input.fields[idx].type;
         const DType& lt = le->lit.type;
         if (ct.is_varlen() || ct.id == T_NULL) return false;
+        // the VM compares a timestamp only with a timestamp of the same unit (raw numbers of two units mean different instants)
+        if ((ct.id == T_TIMESTAMP || lt.id == T_TIMESTAMP) && !(lt == ct)) return false;
         int vt = vt_of(ct);
         if (ct.id == T_DECIMAL128) {
             if (!(lt == ct)) return false;
