@@ -56,9 +56,12 @@ enum Op : uint16_t {
     OP_OUT, OP_OUT_PRED, OP_FMT_OUT,
     OP_SB_BEGIN, OP_SB_APPEND, OP_SB_END,
 };
-// OP_SB_APPEND: flags = piece kind | SB_WS (concat_ws) | SB_REPEAT; aux = output | constant << 8 (the separator with SB_WS, the
-// count with SB_REPEAT); aux2 = FmtKind << 8 | scale of an SB_FMT piece
+// OP_SB_APPEND: flags = piece kind | SB_WS (concat_ws) | SB_REPEAT | SbFn << 4 (a string function of the view in a, with its
+// arguments in b and c); aux = output | constant << 8 (the separator with SB_WS, the count with SB_REPEAT); aux2 = FmtKind << 8 |
+// scale of an SB_FMT piece
 enum SbPiece : int { SB_VIEW = 0, SB_FMT = 1, SB_SPACE = 2, SB_WS = 4, SB_REPEAT = 8 };
+enum CharlenFlags : int { CL_CHARS = 0, CL_ASCII = 1, CL_FIND_IN_SET = 2 };
+constexpr int TRIM_SET = 4;   // OP_TRIM flag: trim the characters of the view in b instead of ASCII spaces
 enum DatePart : int { DP_YEAR = 0, DP_MONTH, DP_DAY, DP_DOW, DP_QUARTER, DP_WEEK, DP_DOY };
 enum Math1 : int { M_SQRT = 0, M_EXP, M_LN, M_LOG10, M_LOG2, M_SIN, M_COS, M_TAN, M_ASIN, M_ACOS, M_ATAN, M_CEIL, M_FLOOR, M_SIGNUM, M_TRUNC, M_EXPM1 };
 
@@ -746,6 +749,183 @@ __device__ __forceinline__ void copy_view(uint8_t* d, const uint8_t* s, int32_t 
     }
 }
 
+// ------------------------------------------------------------------------------------------ string functions
+// A character is a lead byte and the continuation bytes it announces, cut at the end of the view (as OP_SUBSTR counts them).
+// Every byte is read through the view's ASCII upper / lower mark, so that matching sees the bytes copying writes.
+struct SView {
+    const uint8_t* p;
+    int32_t n;
+    int xf;
+    __device__ __forceinline__ uint8_t at(int32_t k) const {
+        uint8_t c = p[k];
+        if (xf == 1 && c >= 'a' && c <= 'z') c -= 32;
+        else if (xf == 2 && c >= 'A' && c <= 'Z') c += 32;
+        return c;
+    }
+    __device__ __forceinline__ int32_t clen(int32_t k) const {   // bytes of the character that starts at k
+        const int32_t l = utf8_char_len(p[k]);
+        return l < n - k ? l : n - k;
+    }
+};
+__device__ __forceinline__ SView sview(const VmParams& p, int64_t h, uint64_t x) { return {str_ptr(p, h, x), str_len(x), (int)((h >> 8) & 0xff)}; }
+__device__ __forceinline__ bool sv_eq(const SView& a, int32_t i, const SView& b, int32_t j, int32_t len) {
+    for (int32_t k = 0; k < len; k++)
+        if (a.at(i + k) != b.at(j + k)) return false;
+    return true;
+}
+// the index (in characters) of the first character of `set` equal to a[i, i + len), -1 when there is none
+__device__ inline int32_t sv_char_index(const SView& set, const SView& a, int32_t i, int32_t len) {
+    int32_t k = 0;
+    for (int32_t j = 0; j < set.n; k++) {
+        const int32_t cl = set.clen(j);
+        if (cl == len && sv_eq(set, j, a, i, len)) return k;
+        j += cl;
+    }
+    return -1;
+}
+// trim with a character set (DataFusion btrim / ltrim / rtrim with a second argument): sides 1 = leading, 2 = trailing
+__device__ inline void trim_set(const SView& s, const SView& set, int sides, int32_t* b, int32_t* e) {
+    if (sides & 1)
+        while (*b < *e) {
+            const int32_t cl = s.clen(*b);
+            if (sv_char_index(set, s, *b, cl) < 0) break;
+            *b += cl;
+        }
+    if (sides & 2)
+        while (*e > *b) {
+            int32_t j = *e - 1;
+            while (j > *b && (s.p[j] & 0xc0) == 0x80) j--;
+            if (sv_char_index(set, s, j, *e - j) < 0) break;
+            *e = j;
+        }
+}
+// ascii(s): the code point of the first character, 0 for ""
+__device__ inline int32_t str_ascii(const SView& s) {
+    if (s.n == 0) return 0;
+    const int32_t cl = s.clen(0);
+    int32_t r = s.at(0);
+    if (cl > 1) {
+        r &= 0x7f >> cl;
+        for (int32_t k = 1; k < cl; k++) r = (r << 6) | (s.p[k] & 0x3f);
+    }
+    return r;
+}
+// find_in_set(a, list) (Spark UTF8String.findInSet): the 1-based index of `a` among the comma-separated pieces of `list`; 0 when
+// `a` holds a comma or is not there
+__device__ inline int32_t str_find_in_set(const SView& a, const SView& list) {
+    for (int32_t k = 0; k < a.n; k++)
+        if (a.at(k) == ',') return 0;
+    int32_t idx = 1, start = 0;
+    for (int32_t j = 0; j <= list.n; j++) {
+        if (j < list.n && list.at(j) != ',') continue;
+        if (j - start == a.n && sv_eq(list, start, a, 0, a.n)) return idx;
+        idx++;
+        start = j + 1;
+    }
+    return 0;
+}
+
+// A builder row's length saturates here, so that no row wraps the int64 scan of the lengths; such a row fails its batch's 2 GiB check.
+constexpr int64_t SB_SAT = (int64_t)INT32_MAX + 1;
+// the string functions the builder runs as pieces (OP_SB_APPEND flags >> 4); the first four take three arguments
+enum SbFn : int { SBF_NONE = 0, SBF_LPAD, SBF_RPAD, SBF_REPLACE, SBF_TRANSLATE, SBF_REVERSE, SBF_INITCAP };
+
+// One string-function piece of s: lpad / rpad to n characters with pad x, replace search x by y, translate characters of x into
+// those of y, reverse, initcap.  Returns its byte length (above SB_SAT only when the row is too long anyway); with d (pass 1) it
+// also writes the piece there.
+__device__ inline int64_t sb_fn_piece(int fn, const SView& s, const SView& x, const SView& y, int64_t n, uint8_t* d) {
+    switch (fn) {
+        case SBF_LPAD: case SBF_RPAD: {   // Spark UTF8String.lpad / rpad
+            if (n <= 0) return 0;
+            int32_t sb = 0;   // bytes of s's first n characters
+            int64_t ch = 0;
+            while (sb < s.n && ch < n) {
+                sb += s.clen(sb);
+                ch++;
+            }
+            if (ch == n || x.n == 0) {   // truncated to n characters, or nothing to pad with
+                if (d) copy_view(d, s.p, sb, s.xf);
+                return sb;
+            }
+            int64_t pc = 0;
+            for (int32_t j = 0; j < x.n; j += x.clen(j)) pc++;
+            const int64_t q = (n - ch) / pc, r = (n - ch) % pc;   // n - ch pad characters: q whole pads and r more
+            int32_t rb = 0;
+            for (int64_t c = 0; c < r; c++) rb += x.clen(rb);
+            if (q > (SB_SAT - sb - rb) / x.n) return SB_SAT;
+            if (d) {
+                uint8_t* pd = fn == SBF_LPAD ? d : d + sb;
+                for (int64_t c = 0; c < q; c++) copy_view(pd + c * x.n, x.p, x.n, x.xf);
+                copy_view(pd + q * x.n, x.p, rb, x.xf);
+                copy_view(fn == SBF_LPAD ? d + q * x.n + rb : d, s.p, sb, s.xf);
+            }
+            return sb + q * x.n + rb;
+        }
+        case SBF_REPLACE: {   // Spark UTF8String.replace: matches left to right, not overlapping; an empty search changes nothing
+            if (x.n == 0) {
+                if (d) copy_view(d, s.p, s.n, s.xf);
+                return s.n;
+            }
+            int64_t o = 0;
+            for (int32_t i = 0; i < s.n;) {
+                if (i <= s.n - x.n && sv_eq(s, i, x, 0, x.n)) {
+                    if (d) copy_view(d + o, y.p, y.n, y.xf);
+                    o += y.n;
+                    i += x.n;
+                } else {
+                    if (d) d[o] = s.at(i);
+                    o++;
+                    i++;
+                }
+            }
+            return o;
+        }
+        case SBF_TRANSLATE: {   // Spark StringTranslate: the k-th character of x becomes the k-th of y, or is deleted when y is shorter;
+                                // a character repeated in x keeps its first position
+            int64_t o = 0;
+            for (int32_t i = 0; i < s.n;) {
+                const int32_t cl = s.clen(i);
+                const int32_t k = sv_char_index(x, s, i, cl);
+                if (k < 0) {
+                    if (d) copy_view(d + o, s.p + i, cl, s.xf);
+                    o += cl;
+                } else {
+                    int32_t j = 0;
+                    for (int32_t c = 0; j < y.n && c < k; c++) j += y.clen(j);
+                    if (j < y.n) {
+                        const int32_t tl = y.clen(j);
+                        if (d) copy_view(d + o, y.p + j, tl, y.xf);
+                        o += tl;
+                    }
+                }
+                i += cl;
+            }
+            return o;
+        }
+        case SBF_REVERSE:
+            if (d)
+                for (int32_t i = 0; i < s.n;) {
+                    const int32_t cl = s.clen(i);
+                    copy_view(d + s.n - i - cl, s.p + i, cl, s.xf);
+                    i += cl;
+                }
+            return s.n;
+        default:   // SBF_INITCAP, spark_initcap.rs:40-66 for ASCII: a letter or digit first or after ' ' upper-cased, every other
+                   // letter lower-cased; other bytes copied
+            if (d) {
+                bool after_space = true;
+                for (int32_t i = 0; i < s.n; i++) {
+                    uint8_t c = s.at(i);
+                    if (after_space && c >= 'a' && c <= 'z') c -= 32;
+                    else if (!after_space && c >= 'A' && c <= 'Z') c += 32;
+                    d[i] = c;
+                    after_space = c == ' ';
+                }
+            }
+            return s.n;
+    }
+}
+
 template <bool HI>
 __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
     extern __shared__ __align__(16) uint64_t vm_smem[];
@@ -1016,13 +1196,16 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                     SETV(ins.dst, v);
                     break;
                 }
-                case OP_CHARLEN: case OP_OCTLEN: {
+                case OP_CHARLEN: case OP_OCTLEN: {   // OP_CHARLEN flags: CL_CHARS, CL_ASCII, CL_FIND_IN_SET (the list in b)
                     bool v = VALID(ins.a);
+                    if (HI && ins.flags == CL_FIND_IN_SET) v = v && VALID(ins.b);
                     int64_t r = 0;
                     if (HI && v) {
                         uint64_t sv = RLO(ins.a);
                         int32_t ls = str_len(sv);
                         if (ins.op == OP_OCTLEN) r = ls;
+                        else if (ins.flags == CL_ASCII) r = str_ascii(sview(p, RHI(ins.a), sv));
+                        else if (ins.flags == CL_FIND_IN_SET) r = str_find_in_set(sview(p, RHI(ins.a), sv), sview(p, RHI(ins.b), RLO(ins.b)));
                         else {
                             const uint8_t* s = str_ptr(p, RHI(ins.a), sv);
                             for (int32_t k = 0; k < ls; k++) r += (s[k] & 0xc0) != 0x80;
@@ -1032,15 +1215,19 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                     SETV(ins.dst, v);
                     break;
                 }
-                case OP_TRIM: {   // flags: 1 = left, 2 = right ; trims ASCII space
+                case OP_TRIM: {   // flags: 1 = left, 2 = right ; trims ASCII space, or with TRIM_SET the characters of the view in b
                     bool v = VALID(ins.a);
+                    if (HI && (ins.flags & TRIM_SET)) v = v && VALID(ins.b);
                     uint64_t sv = RLO(ins.a);
                     int64_t h = HI ? RHI(ins.a) : 0;
                     if (HI && v) {
                         const uint8_t* s = str_ptr(p, h, sv);
                         int32_t b = 0, e = str_len(sv);
-                        if (ins.flags & 1) while (b < e && s[b] == ' ') b++;
-                        if (ins.flags & 2) while (e > b && s[e - 1] == ' ') e--;
+                        if (ins.flags & TRIM_SET) trim_set(sview(p, h, sv), sview(p, RHI(ins.b), RLO(ins.b)), ins.flags, &b, &e);
+                        else {
+                            if (ins.flags & 1) while (b < e && s[b] == ' ') b++;
+                            if (ins.flags & 2) while (e > b && s[e - 1] == ' ') e--;
+                        }
                         sv = ((uint64_t)((uint32_t)(sv >> 32) + (uint32_t)b) << 32) | (uint32_t)(e - b);
                     }
                     RLO(ins.dst) = sv;
@@ -1302,8 +1489,9 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                 }
                 case OP_SB_APPEND: {
                     if (!HI || !VALID(ins.dst)) break;
-                    const int kind = ins.flags & 3;
-                    if (!VALID(ins.a)) {   // concat: a NULL piece makes the row NULL; concat_ws skips it
+                    const int kind = ins.flags & 3, fn = ins.flags >> 4;
+                    if (!VALID(ins.a) || (fn >= SBF_LPAD && fn <= SBF_TRANSLATE && !(VALID(ins.b) && VALID(ins.c)))) {
+                        // concat: a NULL piece (a string function with a NULL argument) makes the row NULL; concat_ws skips it
                         if (!(ins.flags & SB_WS)) SETV(ins.dst, false);
                         break;
                     }
@@ -1322,6 +1510,17 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                         if (d)
                             for (int64_t k = 0; k < n; k++) d[cur + k] = ' ';
                         cur += n;
+                    } else if (fn != SBF_NONE) {   // lpad / rpad: b = length, c = pad; replace / translate: b, c; others: s only
+                        SView u{nullptr, 0, 0}, w{nullptr, 0, 0};
+                        int64_t n = 0;
+                        if (fn <= SBF_RPAD) {
+                            n = (int64_t)RLO(ins.b);
+                            u = sview(p, RHI(ins.c), RLO(ins.c));
+                        } else if (fn <= SBF_TRANSLATE) {
+                            u = sview(p, RHI(ins.b), RLO(ins.b));
+                            w = sview(p, RHI(ins.c), RLO(ins.c));
+                        }
+                        cur += sb_fn_piece(fn, sview(p, RHI(ins.a), x), u, w, n, d ? d + cur : nullptr);
                     } else {   // a view or a formatted value, once or `times` times
                         const int64_t times = (ins.flags & SB_REPEAT) ? (int64_t)p.consts[ins.aux >> 8].lo : 1;
                         const uint8_t* s;
@@ -1339,7 +1538,7 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                         for (int64_t r = 0; d && r < times; r++) copy_view(d + cur + r * len, s, len, xf);
                         cur += times * len;
                     }
-                    RLO(ins.dst) = (uint64_t)cur;
+                    RLO(ins.dst) = (uint64_t)(cur < SB_SAT ? cur : SB_SAT);
                     break;
                 }
                 case OP_SB_END: {
@@ -1674,7 +1873,13 @@ static int digest_alg_of(const std::string& f) {
     return f == "Spark_MD5" ? DIGEST_MD5 : f == "Spark_Sha224" ? DIGEST_SHA224 : f == "Spark_Sha256" ? DIGEST_SHA256 :
            f == "Spark_Sha384" ? DIGEST_SHA384 : f == "Spark_Sha512" ? DIGEST_SHA512 : 0;
 }
-bool makes_string_fn(const std::string& f) { return is_string_builder(f) || digest_alg_of(f) != 0; }
+// the string functions the builder runs as one piece (NativeConverters.scala:902-905,929-932,1053-1062): a whole projection
+// expression, a piece of concat / concat_ws or a digest's argument
+static int string_fn_of(const std::string& f) {
+    return f == "Lpad" ? SBF_LPAD : f == "Rpad" ? SBF_RPAD : f == "Replace" ? SBF_REPLACE : f == "Translate" ? SBF_TRANSLATE :
+           f == "Reverse" ? SBF_REVERSE : f == "Spark_InitCap" ? SBF_INITCAP : SBF_NONE;
+}
+bool makes_string_fn(const std::string& f) { return is_string_builder(f) || digest_alg_of(f) != 0 || string_fn_of(f) != SBF_NONE; }
 static bool makes_string(const Expr& e) { return e.kind == E_SCALAR_FN && makes_string_fn(e.name); }
 // the planner's declared-type TRY_CAST around one of them (operators.cc ProjectExec) is the identity: their type is utf8
 static const Expr& strip_utf8_cast(const Expr& e) {
@@ -1985,7 +2190,15 @@ struct Compiler {
             emit(OP_TIMEPART, a.reg, a.reg, 0, 0, VT_I32, 0, which);
             return Val{a.reg, DType(T_INT32)};
         };
+        if (string_fn_of(f) != SBF_NONE)
+            fail(f + " is only native as a whole projection expression, a piece of concat / concat_ws or the argument of md5 / sha2");
         if (makes_string(e)) fail(f + " is only native as a whole projection expression or as the argument of md5 / sha2");
+        // a utf8 argument of a string function (a NULL literal gives NULL)
+        auto text_arg = [&](const Expr& x) {
+            Val v = gen(x);
+            if (v.type.id != T_UTF8 && v.type.id != T_NULL) fail(f + " argument of type " + v.type.str() + " is not native (utf8 only)");
+            return v;
+        };
         Val r{-1, DType()};
         if (f == "Spark_Year") r = date_fn(DP_YEAR);
         else if (f == "Spark_Month") r = date_fn(DP_MONTH);
@@ -2092,10 +2305,34 @@ struct Compiler {
             Val s = gen(*e.children[0]);
             emit(f == "CharacterLength" ? OP_CHARLEN : OP_OCTLEN, s.reg, s.reg);
             r = Val{s.reg, DType(T_INT32)};
-        } else if (f == "Trim" || f == "Btrim" || f == "Ltrim" || f == "Rtrim") {
-            AURON_CHECK(e.children.size() == 1, "trim with a custom character set is not native");
+        } else if (f == "Ascii" || f == "FindInSet") {   // int32: the first code point / the index of a in the list b
+            Val s = text_arg(*e.children[0]);
+            if (f == "Ascii") emit(OP_CHARLEN, s.reg, s.reg, 0, 0, VT_STR, CL_ASCII);
+            else {
+                AURON_CHECK(e.children.size() == 2, f + " takes two arguments");
+                Val l = text_arg(*e.children[1]);
+                emit(OP_CHARLEN, s.reg, s.reg, l.reg, 0, VT_STR, CL_FIND_IN_SET);
+                release(l.reg);
+            }
+            r = Val{s.reg, DType(T_INT32)};
+        } else if (f == "BitLength") {   // int32: 8 x the byte length of a utf8 or binary value
             Val s = gen(*e.children[0]);
-            emit(OP_TRIM, s.reg, s.reg, 0, 0, VT_STR, f == "Ltrim" ? 1 : f == "Rtrim" ? 2 : 3);
+            if (!s.type.is_varlen() && s.type.id != T_NULL) fail(f + " argument of type " + s.type.str() + " is not native (utf8 or binary only)");
+            emit(OP_OCTLEN, s.reg, s.reg);
+            Val eight = literal(Literal{DType(T_INT32), false, 8});
+            emit(OP_MUL, s.reg, s.reg, eight.reg, 0, VT_I32);
+            release(eight.reg);
+            r = Val{s.reg, DType(T_INT32)};
+        } else if (f == "Trim" || f == "Btrim" || f == "Ltrim" || f == "Rtrim") {
+            AURON_CHECK(e.children.size() == 1 || e.children.size() == 2, f + " takes one or two arguments");
+            const int sides = f == "Ltrim" ? 1 : f == "Rtrim" ? 2 : 3;
+            Val s = gen(*e.children[0]);
+            if (e.children.size() == 1) emit(OP_TRIM, s.reg, s.reg, 0, 0, VT_STR, sides);
+            else {   // the characters of the second argument
+                Val set = text_arg(*e.children[1]);
+                emit(OP_TRIM, s.reg, s.reg, set.reg, 0, VT_STR, sides | TRIM_SET);
+                release(set.reg);
+            }
             r = s;
         } else if (f == "Upper" || f == "Lower" || f == "Spark_StringUpper" || f == "Spark_StringLower") {
             Val s = gen(*e.children[0]);
@@ -2246,7 +2483,12 @@ struct Compiler {
     }
 
     // one piece of a string constructor: a utf8 value (view), a formatted CAST to utf8, `times` copies of a view, or spaces
-    void append_piece(const std::string& f, int b, int o, const Expr& x, int flags, int const_idx = 0) {
+    void append_piece(const std::string& f, int b, int o, const Expr& x0, int flags, int const_idx = 0) {
+        const Expr& x = strip_utf8_cast(x0);
+        if (x.kind == E_SCALAR_FN && string_fn_of(x.name) != SBF_NONE && !(flags & (SB_REPEAT | SB_SPACE))) {
+            append_fn_piece(x, b, o, flags, const_idx);
+            return;
+        }
         if ((flags & 3) == SB_SPACE) {   // space(n): n is an int32 value, never text
             const DType nt = infer_type(x, in);
             if (nt.id != T_INT32 && nt.id != T_NULL) fail(f + " needs an int32 argument, got " + nt.str());
@@ -2271,6 +2513,38 @@ struct Compiler {
             emit(OP_SB_APPEND, b, v.reg, 0, 0, VT_STR, flags, o | (const_idx << 8));
         }
         release(v.reg);
+    }
+    // lpad / rpad (s, n, pad), replace (s, search, rep), translate (s, from, to), reverse (s), initcap (s) as one piece: every string
+    // argument is any utf8 view, n any integer widened to int64; a NULL argument makes the piece NULL
+    void append_fn_piece(const Expr& x, int b, int o, int flags, int const_idx) {
+        const std::string& g = x.name;
+        const int fn = string_fn_of(g);
+        const size_t nargs = fn <= SBF_TRANSLATE ? 3 : 1;
+        if (x.children.size() != nargs) fail(g + " takes " + std::to_string(nargs) + (nargs == 1 ? " argument" : " arguments"));
+        auto text = [&](const Expr& a) {
+            Val v = gen(a);
+            if (v.type.id != T_UTF8 && v.type.id != T_NULL) fail(g + " argument of type " + v.type.str() + " is not native (utf8 only)");
+            return v;
+        };
+        Val s = text(*x.children[0]);
+        int rb = 0, rc = 0;
+        if (nargs == 3) {
+            Val v1{-1, DType()};
+            if (fn <= SBF_RPAD) {
+                v1 = gen(*x.children[1]);
+                if (!v1.type.is_integer() && v1.type.id != T_NULL) fail(g + " length of type " + v1.type.str() + " is not native (integers only)");
+                v1 = cast_to(v1, DType(T_INT64));
+            } else v1 = text(*x.children[1]);
+            Val v2 = text(*x.children[2]);
+            rb = v1.reg;
+            rc = v2.reg;
+        }
+        emit(OP_SB_APPEND, b, s.reg, rb, rc, VT_STR, SB_VIEW | (flags & SB_WS) | (fn << 4), o | (const_idx << 8));
+        release(s.reg);
+        if (nargs == 3) {
+            release(rb);
+            release(rc);
+        }
     }
     // concat (spark_strings.rs:117-192), concat_ws (:194-319), repeat (:75-91), space (:65-73) into utf8 output `o`.  Each piece is
     // generated, appended and released before the next, so the registers in use do not grow with the number of arguments.
@@ -2306,16 +2580,17 @@ struct Compiler {
             const Literal& n = e.children[1]->lit;
             if (n.is_null) null_row();
             else append_piece(f, b, o, *e.children[0], SB_VIEW | SB_REPEAT, add_const((uint64_t)std::max<int64_t>(0, n.i), 0, true));
-        } else {   // Spark_StringSpace
+        } else if (f == "Spark_StringSpace") {
             if (e.children.size() != 1) fail(f + " takes one argument");
             append_piece(f, b, o, *e.children[0], SB_SPACE);
-        }
+        } else append_fn_piece(e, b, o, SB_VIEW, 0);   // a string function as the whole value
+
         emit(OP_SB_END, 0, b, 0, 0, VT_STR, 0, o);
         release(b);
     }
     // the whole projection expression `ex` into output `o`; returns its type
     DType output(const Expr& ex, int o) {
-        if (ex.kind == E_SCALAR_FN && is_string_builder(ex.name)) {
+        if (ex.kind == E_SCALAR_FN && (is_string_builder(ex.name) || string_fn_of(ex.name) != SBF_NONE)) {
             build_string(ex, o);
             return DType(T_UTF8);
         }

@@ -359,14 +359,15 @@ Literal decode_scalar_ipc(const uint8_t* bytes, size_t n) {
 // ------------------------------------------------------------------------------------------ expressions
 static const char* scalar_fn_name(int fun) {   // auron.proto ScalarFunction :213-292
     switch (fun) {
-        case 0: return "Abs"; case 1: return "Acos"; case 2: return "Asin"; case 3: return "Atan"; case 5: return "Ceil";
-        case 6: return "Cos"; case 8: return "Exp"; case 9: return "Floor"; case 10: return "Ln"; case 11: return "Log";
+        case 0: return "Abs"; case 1: return "Acos"; case 2: return "Asin"; case 3: return "Atan"; case 4: return "Ascii";
+        case 5: return "Ceil"; case 6: return "Cos"; case 8: return "Exp"; case 9: return "Floor"; case 10: return "Ln"; case 11: return "Log";
         case 12: return "Log10"; case 13: return "Log2"; case 14: return "Round"; case 15: return "Signum"; case 16: return "Sin";
-        case 17: return "Sqrt"; case 18: return "Tan"; case 19: return "Trunc"; case 20: return "NullIf"; case 23: return "Btrim";
-        case 24: return "CharacterLength"; case 26: return "Concat"; case 28: return "DatePart"; case 33: return "Lower";
-        case 34: return "Ltrim"; case 37: return "OctetLength"; case 45: return "Rtrim"; case 51: return "StartsWith";
-        case 53: return "Substr"; case 61: return "Trim"; case 62: return "Upper"; case 63: return "Coalesce"; case 64: return "Expm1";
-        case 67: return "Power"; case 69: return "IsNaN"; case 82: return "Nvl";
+        case 17: return "Sqrt"; case 18: return "Tan"; case 19: return "Trunc"; case 20: return "NullIf"; case 22: return "BitLength";
+        case 23: return "Btrim"; case 24: return "CharacterLength"; case 26: return "Concat"; case 28: return "DatePart";
+        case 32: return "Lpad"; case 33: return "Lower"; case 34: return "Ltrim"; case 37: return "OctetLength"; case 41: return "Replace";
+        case 42: return "Reverse"; case 44: return "Rpad"; case 45: return "Rtrim"; case 51: return "StartsWith";
+        case 53: return "Substr"; case 60: return "Translate"; case 61: return "Trim"; case 62: return "Upper"; case 63: return "Coalesce";
+        case 64: return "Expm1"; case 67: return "Power"; case 69: return "IsNaN"; case 81: return "FindInSet"; case 82: return "Nvl";
         default: return nullptr;
     }
 }

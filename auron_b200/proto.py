@@ -157,9 +157,10 @@ def in_list(e: bytes, items: list[bytes], negated: bool = False) -> bytes:
     return f_bytes(13, f_bytes(1, e) + b"".join(f_bytes(2, i) for i in items) + f_varint(3, int(negated)))
 
 
-SCALAR_FN = {"Abs": 0, "Ceil": 5, "Exp": 8, "Floor": 9, "Ln": 10, "Log10": 12, "Log2": 13, "Signum": 15, "Sqrt": 17, "NullIf": 20,
-             "CharacterLength": 24, "DatePart": 28, "Lower": 33, "Ltrim": 34, "OctetLength": 37, "Rtrim": 45, "StartsWith": 51,
-             "Substr": 53, "Trim": 61, "Upper": 62, "Coalesce": 63, "Power": 67, "IsNaN": 69, "AuronExtFunctions": 10000}
+SCALAR_FN = {"Abs": 0, "Ascii": 4, "Ceil": 5, "Exp": 8, "Floor": 9, "Ln": 10, "Log10": 12, "Log2": 13, "Signum": 15, "Sqrt": 17,
+             "NullIf": 20, "BitLength": 22, "CharacterLength": 24, "DatePart": 28, "Lpad": 32, "Lower": 33, "Ltrim": 34, "OctetLength": 37,
+             "Replace": 41, "Reverse": 42, "Rpad": 44, "Rtrim": 45, "StartsWith": 51, "Substr": 53, "Translate": 60, "Trim": 61,
+             "Upper": 62, "Coalesce": 63, "Power": 67, "IsNaN": 69, "FindInSet": 81, "AuronExtFunctions": 10000}
 
 
 def scalar_fn(name: str, args: list[bytes], return_type: pa.DataType) -> bytes:

@@ -8,9 +8,10 @@ north star asks for next to the config-2 bench line; they are not bench.py lines
            d_date_sk int32, d_year int32) on the date key, inner, build = date_dim
   sort     cfg 4 (one GPU's share): ORDER BY ss_item_sk over (ss_item_sk int32, ss_ticket_number int64, ss_ext_sales_price decimal(7,2))
   shuffle  cfg 4: hash repartition of the same rows on ss_item_sk into 200 partitions, compacted shuffle format to /dev/shm
-  strings  md5(s), sha2(s, 256), sha2(s, 512), concat_ws('|', cast(i as string), s) and md5(concat_ws(...)) over N rows of
-           (s utf8, i int64), once with a mean string length of ~32 B and once with ~200 B; each projection feeds a COUNT so that
-           one row leaves the GPU.  Reports compression-function calls per second next to rows/s and input GB/s.
+  strings  md5(s), sha2(s, 256), sha2(s, 512), concat_ws('|', cast(i as string), s), md5(concat_ws(...)), lpad(s, mean, '0'),
+           replace(s, 'a', 'xy'), translate(s, 'abc', 'xy') and initcap(s) over N rows of (s utf8, i int64), once with a mean string
+           length of ~32 B and once with ~200 B; each projection feeds a COUNT so that one row leaves the GPU.  Reports
+           compression-function calls per second next to rows/s and input GB/s.
   filter_project  cfg 1 shape on the expression VM: Project[a + 1, substr(s, 1, 4), CAST(d * 3 AS decimal(38, 2))] <-
            Filter[a > 100000 AND s LIKE 'a%'] over N rows (a int64 1 % NULL, s utf8 4-24 B, d int64), + COUNT / SUM so that one
            row leaves the GPU; the decimal output runs the 128-bit variant of vm_kernel
@@ -171,12 +172,15 @@ if "strings" in which:
         chunk = min(CHUNK, (1 << 31) // (2 * mean + 160))   # keeps every utf8 input and output of one batch below 2 GiB
         pool = rng.integers(32, 127, 1 << 20, dtype=np.uint8)
         lens_all, ws_all = [], []
+        n_a = n_c = 0   # bytes 'a' and 'c' in all values: what replace and translate add and delete
         for start in range(0, N, chunk):
             n = min(chunk, N - start)
             lens = rng.integers(0, 2 * mean + 1, n).astype(np.int64)
             offs = np.zeros(n + 1, dtype=np.int32)
             np.cumsum(lens, out=offs[1:])
             data = np.resize(pool, int(offs[-1]))
+            n_a += int(np.count_nonzero(data == ord("a")))
+            n_c += int(np.count_nonzero(data == ord("c")))
             s_arr = pa.Array.from_buffers(pa.string(), n, [None, pa.py_buffer(offs), pa.py_buffer(data)])
             i_np = rng.integers(-2**62, 2**62, n, dtype=np.int64)
             runtime.put_device_batch(f"str{mean}", pa.record_batch([s_arr, pa.array(i_np)], names=["s", "i"]))
@@ -198,7 +202,15 @@ if "strings" in which:
                   ("digest_sha512", digest_calls(lens, 128, 16))),
                  ("concat_ws('|', cast(i as string), s)", ws, {"expr_vm": s_in + 8 * N + ws_out}, None),
                  ("md5(concat_ws(...))", P.scalar_fn("Spark_MD5", [ws], U), {"expr_vm": s_in + 8 * N + ws_out, "digest_md5": ws_out + hexb(32)},
-                  ("digest_md5", digest_calls(ws_lens, 64, 8)))]
+                  ("digest_md5", digest_calls(ws_lens, 64, 8))),
+                 # the values are ASCII, so characters are bytes: lpad to the mean length writes exactly `mean` bytes per row
+                 (f"lpad(s, {mean}, '0')", P.scalar_fn("Lpad", [P.col("s"), P.lit(mean, pa.int64()), P.lit("0", U)], U),
+                  {"expr_vm": s_in + hexb(mean)}, None),
+                 ("replace(s, 'a', 'xy')", P.scalar_fn("Replace", [P.col("s"), P.lit("a", U), P.lit("xy", U)], U),
+                  {"expr_vm": 2 * s_in + n_a}, None),
+                 ("translate(s, 'abc', 'xy')", P.scalar_fn("Translate", [P.col("s"), P.lit("abc", U), P.lit("xy", U)], U),
+                  {"expr_vm": 2 * s_in - n_c}, None),
+                 ("initcap(s)", P.scalar_fn("Spark_InitCap", [P.col("s")], U), {"expr_vm": 2 * s_in}, None)]
         for label, expr, alg, digest in cases:
             proj = P.projection(P.ffi_reader(schema, f"str{mean}"), [expr], ["h"], [U])
             plan = P.agg(proj, [], [], [P.agg_expr("COUNT", [P.col("h")], pa.int64())], ["c"], ["PARTIAL"])
