@@ -37,6 +37,7 @@ enum ExprKind {
     E_CONTAINS,
     E_SC_AND,
     E_SC_OR,
+    E_ROW_NUM,     // RowNumExprNode: int64 position of the row among the rows the projection emitted (row_num.rs)
 };
 
 struct Expr;
@@ -70,8 +71,9 @@ struct VmProgram {
     std::vector<DType> out_types;   // one per output expression (empty for predicate programs)
     bool is_predicate = false;
 };
-// outputs = projection expressions
-VmProgram compile_projection(const std::vector<ExprPtr>& exprs, const Schema& input);
+// outputs = projection expressions; RowNum is accepted only with `row_num` (a ProjectExec, which passes its row count to
+// eval_projection)
+VmProgram compile_projection(const std::vector<ExprPtr>& exprs, const Schema& input, bool row_num = false);
 // conjunction of predicates; NULL -> false (cached_exprs_evaluator.rs:514-519)
 VmProgram compile_predicate(const std::vector<ExprPtr>& conjuncts, const Schema& input);
 
@@ -79,8 +81,8 @@ VmProgram compile_predicate(const std::vector<ExprPtr>& conjuncts, const Schema&
 // columns): the columns (schema indices) and their bounds in the int64 domain; false when the predicate has another shape
 bool predicate_intervals(const VmProgram& p, std::vector<int>* cols, std::vector<int64_t>* lo, std::vector<int64_t>* hi);
 
-// evaluate over rows sel[0..n_out) (sel == nullptr: rows 0..n_out)
-std::vector<ColumnPtr> eval_projection(Ctx& ctx, const VmProgram& p, const Batch& in, const int32_t* sel, int64_t n_out);
+// evaluate over rows sel[0..n_out) (sel == nullptr: rows 0..n_out); RowNum gives row_base + the row's output position
+std::vector<ColumnPtr> eval_projection(Ctx& ctx, const VmProgram& p, const Batch& in, const int32_t* sel, int64_t n_out, int64_t row_base = 0);
 // returns selection bitmap (whole 32-bit words) over the n_rows input rows
 Buf eval_predicate(Ctx& ctx, const VmProgram& p, const Batch& in, int64_t n_rows);
 

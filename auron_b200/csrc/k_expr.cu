@@ -53,6 +53,7 @@ enum Op : uint16_t {
     OP_DATEPART, OP_TS_LOCAL_MS, OP_TIMEPART, OP_MS_TO_DAYS, OP_ROUND, OP_NULLIFZERO, OP_ISNAN, OP_NORMNAN, OP_CHECK_OVERFLOW, OP_MAKE_DECIMAL, OP_UNSCALED,
     OP_MATH1, OP_POW, OP_HASH,
     OP_BITAND, OP_BITOR, OP_BITXOR, OP_SHL, OP_SHR,
+    OP_GREATEST, OP_DATE_TRUNC, OP_MAKE_DATE, OP_FACTORIAL, OP_ROWNUM, OP_MONTHS_BETWEEN,
     OP_OUT, OP_OUT_PRED, OP_FMT_OUT,
     OP_SB_BEGIN, OP_SB_APPEND, OP_SB_END,
 };
@@ -63,7 +64,9 @@ enum SbPiece : int { SB_VIEW = 0, SB_FMT = 1, SB_SPACE = 2, SB_WS = 4, SB_REPEAT
 enum CharlenFlags : int { CL_CHARS = 0, CL_ASCII = 1, CL_FIND_IN_SET = 2 };
 constexpr int TRIM_SET = 4;   // OP_TRIM flag: trim the characters of the view in b instead of ASCII spaces
 enum DatePart : int { DP_YEAR = 0, DP_MONTH, DP_DAY, DP_DOW, DP_QUARTER, DP_WEEK, DP_DOY };
-enum Math1 : int { M_SQRT = 0, M_EXP, M_LN, M_LOG10, M_LOG2, M_SIN, M_COS, M_TAN, M_ASIN, M_ACOS, M_ATAN, M_CEIL, M_FLOOR, M_SIGNUM, M_TRUNC, M_EXPM1 };
+enum Math1 : int { M_SQRT = 0, M_EXP, M_LN, M_LOG10, M_LOG2, M_SIN, M_COS, M_TAN, M_ASIN, M_ACOS, M_ATAN, M_CEIL, M_FLOOR, M_SIGNUM, M_TRUNC, M_EXPM1, M_ACOSH };
+// date_trunc levels, finest first (Spark's TruncTimestamp format names)
+enum TruncLevel : int { TL_MICROSECOND = 0, TL_MILLISECOND, TL_SECOND, TL_MINUTE, TL_HOUR, TL_DAY, TL_WEEK, TL_MONTH, TL_QUARTER, TL_YEAR };
 
 struct Instr {
     uint16_t op;
@@ -90,6 +93,7 @@ struct VmParams {
     const int32_t* sel;
     uint32_t* pred_out;
     int64_t n;
+    int64_t row_base;   // OP_ROWNUM: rows the projection emitted before this launch
     int32_t n_instr;
     int32_t mode;   // 0 eval (fixed outputs + string lengths), 1 copy string bytes
 };
@@ -319,23 +323,116 @@ __device__ inline double powi10(int n) {
 // E4 with a session time zone (spark_dates.rs:200-227,313-345): `v` in `unit` (0 s, 1 ms, 2 us, 3 ns, 4 = Date32 days) becomes
 // Timestamp(Millisecond) the way arrow's cast does it (division truncates toward zero), then the zone's UTC offset at that
 // instant is added.  The zone is a table in the constant pool: int64 n | int64 transition_second[n] | int32 offset[n + 1].
-__device__ inline int64_t ts_to_local_ms(int64_t v, int unit, const uint8_t* tz) {
-    int64_t ms = unit == 0 ? v * 1000 : unit == 1 ? v : unit == 2 ? v / 1000 : unit == 3 ? v / 1000000 : v * 86400000ll;
-    if (tz) {
-        const int64_t n = *(const int64_t*)tz;
-        const int64_t* trans = (const int64_t*)tz + 1;
-        const int32_t* offs = (const int32_t*)(trans + n);
-        // chrono: Utc.timestamp_millis_opt(ms) -> the instant's second is floor(ms / 1000)
-        const int64_t sec = ms >= 0 ? ms / 1000 : -((-ms + 999) / 1000);
-        int64_t lo = 0, hi = n;
-        while (lo < hi) {
-            const int64_t mid = (lo + hi) >> 1;
-            if (trans[mid] <= sec) lo = mid + 1;
-            else hi = mid;
-        }
-        ms += (int64_t)offs[lo] * 1000;
+// the number of transitions of zone table `tz` at or before UTC second `sec`: the index of its offset
+__device__ __forceinline__ int64_t tz_interval(const uint8_t* tz, int64_t sec) {
+    const int64_t n = *(const int64_t*)tz;
+    const int64_t* trans = (const int64_t*)tz + 1;
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (trans[mid] <= sec) lo = mid + 1;
+        else hi = mid;
     }
+    return lo;
+}
+__device__ __forceinline__ int32_t tz_offset(const uint8_t* tz, int64_t k) { return ((const int32_t*)((const int64_t*)tz + 1 + *(const int64_t*)tz))[k]; }
+__device__ __forceinline__ int64_t ts_to_utc_ms(int64_t v, int unit) {
+    return unit == 0 ? v * 1000 : unit == 1 ? v : unit == 2 ? v / 1000 : unit == 3 ? v / 1000000 : v * 86400000ll;
+}
+__device__ __forceinline__ int64_t floor_div(int64_t a, int64_t b) { return a / b - (a % b != 0 && (a < 0) != (b < 0)); }
+__device__ inline int64_t ts_to_local_ms(int64_t v, int unit, const uint8_t* tz) {
+    int64_t ms = ts_to_utc_ms(v, unit);
+    // chrono: Utc.timestamp_millis_opt(ms) -> the instant's second is floor(ms / 1000)
+    if (tz) ms += (int64_t)tz_offset(tz, tz_interval(tz, floor_div(ms, 1000))) * 1000;
     return ms;
+}
+// Local to UTC on zone table `tz` (start_of_local_day_ms, spark_dates.rs:112-139): the earliest UTC second whose local time is
+// `local_s`; when that local time falls into a gap, the earliest one of the first whole minute after it that exists (at most a day
+// later).  false when there is none.  Interval k (offset o, UTC [trans[k - 1], trans[k])) holds the local times
+// [trans[k - 1] + o, trans[k] + o), so its first minute is found without walking; offsets lie within +-26 h, so only the intervals
+// that cover [local_s - 26 h, local_s + 50 h] can hold the answer.  Out of line: inlined, it makes vm_kernel<true> spill.
+__device__ __noinline__ bool local_to_utc_s(const uint8_t* tz, int64_t local_s, int64_t* out) {
+    const int64_t n = *(const int64_t*)tz;
+    const int64_t* trans = (const int64_t*)tz + 1;
+    const int64_t k0 = tz_interval(tz, local_s - 93600), k1 = tz_interval(tz, local_s + 180000);
+    int64_t best = 24 * 60 + 1;
+    for (int64_t k = k0; k <= k1; k++) {   // ascending intervals: at an equal minute the first fit is the earliest instant
+        const int64_t o = tz_offset(tz, k);
+        const int64_t m = k > 0 && trans[k - 1] + o > local_s ? (trans[k - 1] + o - local_s + 59) / 60 : 0;
+        if (m < best && (k == n || local_s + 60 * m < trans[k] + o)) {
+            best = m;
+            *out = local_s + 60 * m - o;
+        }
+    }
+    return best <= 24 * 60;
+}
+__device__ __forceinline__ int days_in_month(int64_t y, unsigned m) {
+    const bool leap = (y % 4 == 0 && y % 100 != 0) || y % 400 == 0;
+    return m == 2 ? 28 + leap : (m == 4 || m == 6 || m == 9 || m == 11) ? 30 : 31;
+}
+// months_between_value (spark_dates.rs:158-198) of two UTC millisecond instants with the zone table `tz` (nullptr: UTC)
+__device__ inline bool months_between(int64_t ms1, int64_t ms2, bool round_off, const uint8_t* tz, double* out) {
+    const int64_t l1 = tz ? ts_to_local_ms(ms1, 1, tz) : ms1, l2 = tz ? ts_to_local_ms(ms2, 1, tz) : ms2;
+    const int64_t day1 = floor_div(l1, 86400000), day2 = floor_div(l2, 86400000);
+    int64_t y1, y2;
+    unsigned m1, d1, m2, d2;
+    civil_from_days(day1, &y1, &m1, &d1);
+    civil_from_days(day2, &y2, &m2, &d2);
+    const double month_diff = (double)((y1 * 12 + m1) - (y2 * 12 + m2));
+    if (d1 == d2 || (d1 == (unsigned)days_in_month(y1, m1) && d2 == (unsigned)days_in_month(y2, m2))) {
+        *out = month_diff;
+        return true;
+    }
+    int64_t s1 = day1 * 86400, s2 = day2 * 86400;   // local midnights, then their UTC instants
+    if (tz && !(local_to_utc_s(tz, s1, &s1) && local_to_utc_s(tz, s2, &s2))) return false;
+    const int64_t secs = ((int64_t)d1 - (int64_t)d2) * 86400 + (ms1 - s1 * 1000) / 1000 - (ms2 - s2 * 1000) / 1000;
+    const double r = month_diff + (double)secs / 2678400.0;
+    *out = round_off ? floor(__dadd_rn(__dmul_rn(r, 1e8), 0.5)) / 1e8 : r;   // two roundings, as Rust does it: no fused multiply-add
+    return true;
+}
+// date_trunc(level, v) of a timestamp in `unit` (0 s .. 3 ns) toward -inf, converted to `out_unit` as arrow's cast does (a coarser
+// unit divides toward zero); false when the result leaves int64
+__device__ inline bool date_trunc(int64_t v, int unit, int level, int out_unit, int64_t* out) {
+    const int64_t unit_ns = unit == 0 ? 1000000000 : unit == 1 ? 1000000 : unit == 2 ? 1000 : 1;
+    const int64_t day = 86400000000000ll / unit_ns;   // units per day
+    int64_t r;
+    if (level <= TL_DAY) {
+        const int64_t step_ns[6] = {1000, 1000000, 1000000000, 60000000000ll, 3600000000000ll, 86400000000000ll};
+        const int64_t step = step_ns[level] > unit_ns ? step_ns[level] / unit_ns : 1;
+        int64_t m = v % step;
+        if (m < 0) m += step;
+        if ((uint64_t)v - (uint64_t)INT64_MIN < (uint64_t)m) return false;
+        r = v - m;
+    } else {
+        int64_t d = floor_div(v, day), y;
+        unsigned mo, dd;
+        civil_from_days(d, &y, &mo, &dd);
+        if (level == TL_WEEK) {   // Monday: day 0 (1970-01-01) is a Thursday
+            int64_t wd = (d + 3) % 7;
+            d -= wd < 0 ? wd + 7 : wd;
+        } else d = days_from_civil_d(y, level == TL_YEAR ? 1 : level == TL_QUARTER ? (mo - 1) / 3 * 3 + 1 : mo, 1);
+        const __int128 w = (__int128)d * day;
+        if (w < INT64_MIN) return false;
+        r = (int64_t)w;
+    }
+    if (out_unit > unit) {
+        int64_t f = 1;
+        for (int k = unit; k < out_unit; k++) f *= 1000;
+        const __int128 w = (__int128)r * f;
+        if (w < INT64_MIN || w > INT64_MAX) return false;
+        r = (int64_t)w;
+    } else
+        for (int k = out_unit; k < unit; k++) r /= 1000;
+    *out = r;
+    return true;
+}
+// make_date(y, m, d): the day number of a valid proleptic Gregorian date that fits int32 (Spark's non-ANSI MakeDate gives NULL otherwise)
+__device__ inline bool make_date(int64_t y, int64_t m, int64_t d, int64_t* out) {
+    if (m < 1 || m > 12 || d < 1 || d > days_in_month(y, (unsigned)m)) return false;
+    const int64_t z = days_from_civil_d(y, (unsigned)m, (unsigned)d);
+    if (z < INT32_MIN || z > INT32_MAX) return false;
+    *out = z;
+    return true;
 }
 
 __device__ __forceinline__ const uint8_t* str_ptr(const VmParams& p, int64_t bufid, uint64_t view) {
@@ -768,6 +865,16 @@ struct SView {
     }
 };
 __device__ __forceinline__ SView sview(const VmParams& p, int64_t h, uint64_t x) { return {str_ptr(p, h, x), str_len(x), (int)((h >> 8) & 0xff)}; }
+// unsigned byte order, the shorter prefix first
+__device__ inline int sv_cmp(const SView& a, const SView& b) {
+    if (a.xf == 0 && b.xf == 0) return str_cmp(a.p, a.n, b.p, b.n);
+    const int32_t n = a.n < b.n ? a.n : b.n;
+    for (int32_t k = 0; k < n; k++) {
+        const uint8_t x = a.at(k), y = b.at(k);
+        if (x != y) return x < y ? -1 : 1;
+    }
+    return a.n == b.n ? 0 : (a.n < b.n ? -1 : 1);
+}
 __device__ __forceinline__ bool sv_eq(const SView& a, int32_t i, const SView& b, int32_t j, int32_t len) {
     for (int32_t k = 0; k < len; k++)
         if (a.at(i + k) != b.at(j + k)) return false;
@@ -827,14 +934,44 @@ __device__ inline int32_t str_find_in_set(const SView& a, const SView& list) {
 
 // A builder row's length saturates here, so that no row wraps the int64 scan of the lengths; such a row fails its batch's 2 GiB check.
 constexpr int64_t SB_SAT = (int64_t)INT32_MAX + 1;
-// the string functions the builder runs as pieces (OP_SB_APPEND flags >> 4); the first four take three arguments
-enum SbFn : int { SBF_NONE = 0, SBF_LPAD, SBF_RPAD, SBF_REPLACE, SBF_TRANSLATE, SBF_REVERSE, SBF_INITCAP };
+// the string functions the builder runs as pieces (OP_SB_APPEND flags >> 4); the first four take three arguments; SBF_HEX_INT and
+// SBF_CHR take an int64 instead of a view
+enum SbFn : int { SBF_NONE = 0, SBF_LPAD, SBF_RPAD, SBF_REPLACE, SBF_TRANSLATE, SBF_REVERSE, SBF_INITCAP, SBF_HEX, SBF_HEX_INT, SBF_CHR };
 
 // One string-function piece of s: lpad / rpad to n characters with pad x, replace search x by y, translate characters of x into
-// those of y, reverse, initcap.  Returns its byte length (above SB_SAT only when the row is too long anyway); with d (pass 1) it
-// also writes the piece there.
+// those of y, reverse, initcap, hex of s or of n, chr of n.  Returns its byte length (above SB_SAT only when the row is too long
+// anyway); with d (pass 1) it also writes the piece there.
 __device__ inline int64_t sb_fn_piece(int fn, const SView& s, const SView& x, const SView& y, int64_t n, uint8_t* d) {
+    const char* hex_digits = "0123456789ABCDEF";
     switch (fn) {
+        case SBF_HEX:   // Spark Hex of utf8 / binary: two upper-case digits per byte
+            if (d)
+                for (int32_t k = 0; k < s.n; k++) {
+                    const uint8_t c = s.at(k);
+                    d[2 * k] = hex_digits[c >> 4];
+                    d[2 * k + 1] = hex_digits[c & 15];
+                }
+            return 2 * (int64_t)s.n;
+        case SBF_HEX_INT: {   // Spark Hex of a long: the two's complement value in upper-case digits without leading zeros
+            const uint64_t u = (uint64_t)n;
+            const int len = u == 0 ? 1 : (67 - __clzll((long long)u)) / 4;
+            if (d)
+                for (int k = 0; k < len; k++) d[len - 1 - k] = hex_digits[(u >> (4 * k)) & 15];
+            return len;
+        }
+        case SBF_CHR: {   // Spark Chr: "" below 0, else code point n & 0xFF in UTF-8
+            if (n < 0) return 0;
+            const uint8_t c = (uint8_t)(n & 0xff);
+            if (c < 0x80) {
+                if (d) d[0] = c;
+                return 1;
+            }
+            if (d) {
+                d[0] = (uint8_t)(0xc0 | (c >> 6));
+                d[1] = (uint8_t)(0x80 | (c & 0x3f));
+            }
+            return 2;
+        }
         case SBF_LPAD: case SBF_RPAD: {   // Spark UTF8String.lpad / rpad
             if (n <= 0) return 0;
             int32_t sb = 0;   // bytes of s's first n characters
@@ -1063,7 +1200,7 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                     SETV(ins.dst, VALID(ins.a));
                     break;
                 }
-                case OP_EQ: case OP_NE: case OP_LT: case OP_LE: case OP_GT: case OP_GE: case OP_NSEQ: {
+                case OP_EQ: case OP_NE: case OP_LT: case OP_LE: case OP_GT: case OP_GE: case OP_NSEQ: case OP_GREATEST: {
                     bool va = VALID(ins.a), vb = VALID(ins.b);
                     uint64_t a = RLO(ins.a), b = RLO(ins.b);
                     int c = 0;
@@ -1076,7 +1213,16 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                             int64_t x = f64_total(__longlong_as_double((int64_t)a)), y = f64_total(__longlong_as_double((int64_t)b));
                             c = x < y ? -1 : (x > y ? 1 : 0);
                         } else if (t == VT_DEC && HI) c = i128_cmp({a, RHI(ins.a)}, {b, RHI(ins.b)});
-                        else if (t == VT_STR && HI) c = str_cmp(str_ptr(p, RHI(ins.a), a), str_len(a), str_ptr(p, RHI(ins.b), b), str_len(b));
+                        else if (t == VT_STR && HI) c = sv_cmp(sview(p, RHI(ins.a), a), sview(p, RHI(ins.b), b));   // through the case marks
+                    }
+                    if (ins.op == OP_GREATEST) {   // a = the running greatest (flags 0) / least (1): b replaces it when it is strictly
+                                                   // beyond it or a is NULL; a NULL b is skipped
+                        if (vb && (!va || (ins.flags ? c > 0 : c < 0))) {
+                            RLO(ins.dst) = b;
+                            if (HI) RHI(ins.dst) = RHI(ins.b);
+                            SETV(ins.dst, true);
+                        }
+                        break;
                     }
                     bool r = false, v = va && vb;
                     switch (ins.op) {
@@ -1385,6 +1531,7 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                         case M_SIGNUM: r = x > 0 ? 1.0 : (x < 0 ? -1.0 : x); break;
                         case M_TRUNC: r = trunc(x); break;
                         case M_EXPM1: r = expm1(x); break;
+                        case M_ACOSH: r = acosh(x); break;
                     }
                     RLO(ins.dst) = (uint64_t)__double_as_longlong(r);
                     SETV(ins.dst, VALID(ins.a));
@@ -1419,6 +1566,40 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                     }
                     RLO(ins.dst) = h;
                     SETV(ins.dst, true);
+                    break;
+                }
+                // The calendar operations run in vm_kernel<true> only (the compiler sets need_hi for them): in vm_kernel<false> they
+                // would cost every plain numeric program 16 registers.
+                case OP_DATE_TRUNC: {   // aux = TruncLevel, aux2 = unit of the input | unit of the result << 4
+                    int64_t r = 0;
+                    const bool v = HI && VALID(ins.a) && date_trunc((int64_t)RLO(ins.a), ins.aux2 & 15, ins.aux, ins.aux2 >> 4, &r);
+                    RLO(ins.dst) = (uint64_t)r;
+                    SETV(ins.dst, v);
+                    break;
+                }
+                case OP_MAKE_DATE: {   // int32 year a, month b, day c -> date32
+                    int64_t r = 0;
+                    const bool v = HI && VALID(ins.a) && VALID(ins.b) && VALID(ins.c) &&
+                                   make_date((int64_t)RLO(ins.a), (int64_t)RLO(ins.b), (int64_t)RLO(ins.c), &r);
+                    RLO(ins.dst) = (uint64_t)r;
+                    SETV(ins.dst, v);
+                    break;
+                }
+                case OP_FACTORIAL: {   // int32 -> int64, NULL outside 0..20
+                    const int64_t x = (int64_t)RLO(ins.a);
+                    int64_t r = 1;
+                    for (int64_t k = 2; k <= x && k <= 20; k++) r *= k;
+                    RLO(ins.dst) = (uint64_t)r;
+                    SETV(ins.dst, VALID(ins.a) && x >= 0 && x <= 20);
+                    break;
+                }
+                case OP_ROWNUM: RLO(ins.dst) = (uint64_t)(p.row_base + i); SETV(ins.dst, true); break;
+                case OP_MONTHS_BETWEEN: {   // UTC ms a, b, bool roundOff c; aux = pool offset of the zone table (-1: UTC)
+                    double r = 0;
+                    const bool v = HI && VALID(ins.a) && VALID(ins.b) && VALID(ins.c) &&
+                                   months_between((int64_t)RLO(ins.a), (int64_t)RLO(ins.b), RLO(ins.c) != 0, ins.aux >= 0 ? p.pool + ins.aux : nullptr, &r);
+                    RLO(ins.dst) = (uint64_t)__double_as_longlong(r);
+                    SETV(ins.dst, v);
                     break;
                 }
                 case OP_OUT: {
@@ -1510,9 +1691,12 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                         if (d)
                             for (int64_t k = 0; k < n; k++) d[cur + k] = ' ';
                         cur += n;
-                    } else if (fn != SBF_NONE) {   // lpad / rpad: b = length, c = pad; replace / translate: b, c; others: s only
-                        SView u{nullptr, 0, 0}, w{nullptr, 0, 0};
+                    } else if (fn != SBF_NONE) {   // lpad / rpad: b = length, c = pad; replace / translate: b, c; hex / chr of an
+                                                   // integer: a; others: s only
+                        SView s{nullptr, 0, 0}, u{nullptr, 0, 0}, w{nullptr, 0, 0};
                         int64_t n = 0;
+                        if (fn == SBF_HEX_INT || fn == SBF_CHR) n = (int64_t)x;
+                        else s = sview(p, RHI(ins.a), x);
                         if (fn <= SBF_RPAD) {
                             n = (int64_t)RLO(ins.b);
                             u = sview(p, RHI(ins.c), RLO(ins.c));
@@ -1520,7 +1704,7 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                             u = sview(p, RHI(ins.b), RLO(ins.b));
                             w = sview(p, RHI(ins.c), RLO(ins.c));
                         }
-                        cur += sb_fn_piece(fn, sview(p, RHI(ins.a), x), u, w, n, d ? d + cur : nullptr);
+                        cur += sb_fn_piece(fn, s, u, w, n, d ? d + cur : nullptr);
                     } else {   // a view or a formatted value, once or `times` times
                         const int64_t times = (ins.flags & SB_REPEAT) ? (int64_t)p.consts[ins.aux >> 8].lo : 1;
                         const uint8_t* s;
@@ -1877,7 +2061,7 @@ static int digest_alg_of(const std::string& f) {
 // expression, a piece of concat / concat_ws or a digest's argument
 static int string_fn_of(const std::string& f) {
     return f == "Lpad" ? SBF_LPAD : f == "Rpad" ? SBF_RPAD : f == "Replace" ? SBF_REPLACE : f == "Translate" ? SBF_TRANSLATE :
-           f == "Reverse" ? SBF_REVERSE : f == "Spark_InitCap" ? SBF_INITCAP : SBF_NONE;
+           f == "Reverse" ? SBF_REVERSE : f == "Spark_InitCap" ? SBF_INITCAP : f == "Hex" ? SBF_HEX : f == "Chr" ? SBF_CHR : SBF_NONE;
 }
 bool makes_string_fn(const std::string& f) { return is_string_builder(f) || digest_alg_of(f) != 0 || string_fn_of(f) != SBF_NONE; }
 static bool makes_string(const Expr& e) { return e.kind == E_SCALAR_FN && makes_string_fn(e.name); }
@@ -1936,6 +2120,7 @@ DType infer_type(const Expr& e, const Schema& in) {
         case E_NOT: case E_IS_NULL: case E_IS_NOT_NULL: case E_IN_LIST: case E_LIKE: case E_STARTS_WITH: case E_ENDS_WITH: case E_CONTAINS:
         case E_SC_AND: case E_SC_OR:
             return DType(T_BOOL);
+        case E_ROW_NUM: return DType(T_INT64);
         case E_NEGATIVE: return infer_type(*e.children[0], in);
         case E_CASE: return infer_type(*e.children[e.has_case_expr ? 2 : 1], in);
         case E_CAST: case E_TRY_CAST: return e.type;
@@ -1952,6 +2137,11 @@ struct Compiler {
     VmProgramImpl& prog;
     bool used[VM_NREG] = {false};
     std::map<int, int> col_slot;
+    // RowNum counts the rows a projection emits, so it is valid only where every emitted row evaluates it: in a projection,
+    // outside the branches the reference evaluates on a subset of the rows (CASE results and later conditions, coalesce's later
+    // arguments, the right operand of a short-circuit AND / OR)
+    bool row_num_ok = false;
+    int cond_depth = 0;
 
     Compiler(const Schema& s, VmProgramImpl& p) : in(s), prog(p) {}
     struct Val {
@@ -2119,15 +2309,10 @@ struct Compiler {
             emit(OP_MATH1, a.reg, a.reg, 0, 0, VT_F64, 0, m);
             return Val{a.reg, DType(T_FLOAT64)};
         };
-        // optional second argument: the session time zone as a utf8 literal (spark_dates.rs:93-102); a NULL literal, a
-        // non-literal or a name chrono-tz would not parse means "no zone"
-        auto zone_table = [&](bool* named, std::string* name) -> int {
-            *named = false;
-            if (e.children.size() < 2) return -1;
-            const Expr& z = *e.children[1];
+        // the session time zone as a utf8 literal (spark_dates.rs:93-102) into the pool; a NULL literal, a non-literal or a name
+        // chrono-tz would not parse means "no zone" (-1)
+        auto zone_table_of = [&](const Expr& z) -> int {
             if (z.kind != E_LITERAL || z.lit.is_null || !z.lit.type.is_varlen()) return -1;
-            *named = true;
-            *name = z.lit.s;
             TzTable tab;
             if (!load_tz_table(z.lit.s, &tab)) return -1;
             while (prog.pool.size() % 8) prog.pool.push_back('\0');
@@ -2138,6 +2323,15 @@ struct Compiler {
             prog.pool.append((const char*)tab.offs.data(), (size_t)(n + 1) * 4);
             while (prog.pool.size() % 8) prog.pool.push_back('\0');
             return at;
+        };
+        auto zone_table = [&](bool* named, std::string* name) -> int {   // the optional second argument
+            *named = false;
+            if (e.children.size() < 2) return -1;
+            const Expr& z = *e.children[1];
+            if (z.kind != E_LITERAL || z.lit.is_null || !z.lit.type.is_varlen()) return -1;
+            *named = true;
+            *name = z.lit.s;
+            return zone_table_of(z);
         };
         auto unit_of = [&](const DType& t) -> int {
             if (t.id == T_DATE32) return 4;
@@ -2350,12 +2544,100 @@ struct Compiler {
             r = a;
         } else if (f == "Coalesce" || f == "Nvl") {
             Val a = gen(*e.children[0]);
+            cond_depth++;
             for (size_t k = 1; k < e.children.size(); k++) {
                 Val b = cast_to(gen(*e.children[k]), a.type);
                 emit(OP_COALESCE, a.reg, a.reg, b.reg);
                 release(b.reg);
             }
+            cond_depth--;
             r = a;
+        } else if (f == "Greatest" || f == "Least") {
+            // 2..N arguments of one type, NULLs skipped, the VM's comparison order, the earlier argument on ties; one running value
+            // and one argument live at a time
+            if (e.children.size() < 2) fail(f + " takes at least two arguments");
+            DType rt(T_NULL);
+            for (auto& ch : e.children)
+                if (rt.id == T_NULL) rt = infer_type(*ch, in);
+            if (rt.id == T_NULL) rt = e.type;
+            Val acc{-1, DType()};
+            for (auto& ch : e.children) {
+                Val b = gen(*ch);
+                if (b.type.id == T_NULL) b = cast_to(b, rt);
+                if (b.type != rt) fail(f + " needs arguments of one type, got " + rt.str() + " and " + b.type.str());
+                if (acc.reg < 0) {
+                    acc = b;
+                    continue;
+                }
+                note_type(rt);
+                emit(OP_GREATEST, acc.reg, acc.reg, b.reg, 0, vt_of(rt), f == "Least" ? 1 : 0);
+                release(b.reg);
+            }
+            r = acc;
+        } else if (f == "Nvl2") {   // b when a is not NULL, else c
+            if (e.children.size() != 3) fail(f + " takes three arguments");
+            DType rt = infer_type(*e.children[1], in);
+            if (rt.id == T_NULL) rt = infer_type(*e.children[2], in);
+            if (rt.id == T_NULL) rt = e.type;
+            Val a = gen(*e.children[0]);
+            emit(OP_ISNOTNULL, a.reg, a.reg);
+            Val b = cast_to(gen(*e.children[1]), rt);
+            Val c = cast_to(gen(*e.children[2]), rt);
+            note_type(rt);
+            emit(OP_SELECT, a.reg, a.reg, b.reg, c.reg);
+            release(b.reg);
+            release(c.reg);
+            r = Val{a.reg, rt};
+        } else if (f == "DateTrunc") {   // date_trunc('level', ts): the wall clock of the value as UTC, toward -inf
+            if (e.children.size() != 2) fail("date_trunc takes two arguments");
+            const Expr& fe = *e.children[0];
+            if (fe.kind != E_LITERAL) fail("date_trunc needs a literal format");
+            Val a = gen(*e.children[1]);
+            if (a.type.id != T_TIMESTAMP) fail("date_trunc needs a timestamp argument, got " + a.type.str());
+            const DType rt = e.type.id == T_TIMESTAMP ? e.type : a.type;
+            std::string lv = fe.lit.is_null || !fe.lit.type.is_varlen() ? "" : fe.lit.s;
+            for (auto& ch : lv) ch = (char)toupper(ch);
+            const int level = lv == "YEAR" || lv == "YYYY" || lv == "YY" ? TL_YEAR : lv == "QUARTER" ? TL_QUARTER :
+                              lv == "MONTH" || lv == "MON" || lv == "MM" ? TL_MONTH : lv == "WEEK" ? TL_WEEK : lv == "DAY" || lv == "DD" ? TL_DAY :
+                              lv == "HOUR" ? TL_HOUR : lv == "MINUTE" ? TL_MINUTE : lv == "SECOND" ? TL_SECOND : lv == "MILLISECOND" ? TL_MILLISECOND :
+                              lv == "MICROSECOND" ? TL_MICROSECOND : -1;
+            if (level < 0) emit(OP_CONST, a.reg, 0, 0, 0, 0, 0, add_const(0, 0, false));   // an unknown or NULL format gives NULL
+            else {
+                prog.need_hi = true;
+                emit(OP_DATE_TRUNC, a.reg, a.reg, 0, 0, VT_I64, 0, level, a.type.unit | (rt.unit << 4));
+            }
+            r = Val{a.reg, rt};
+        } else if (f == "MakeDate") {
+            if (e.children.size() != 3) fail("make_date takes three arguments");
+            Val y = cast_to(gen(*e.children[0]), DType(T_INT32));
+            Val m = cast_to(gen(*e.children[1]), DType(T_INT32));
+            Val d = cast_to(gen(*e.children[2]), DType(T_INT32));
+            prog.need_hi = true;
+            emit(OP_MAKE_DATE, y.reg, y.reg, m.reg, d.reg, VT_I32);
+            release(m.reg);
+            release(d.reg);
+            r = Val{y.reg, DType(T_DATE32)};
+        } else if (f == "Factorial") {
+            Val a = gen(*e.children[0]);
+            if (a.type.id != T_INT32 && a.type.id != T_NULL) fail("factorial needs an int32 argument, got " + a.type.str());
+            a = cast_to(a, DType(T_INT32));
+            emit(OP_FACTORIAL, a.reg, a.reg, 0, 0, VT_I64);
+            r = Val{a.reg, DType(T_INT64)};
+        } else if (f == "Spark_MonthsBetween") {
+            // spark_months_between (spark_dates.rs:403-458): both timestamps cast to Timestamp(ms), roundOff to bool, the zone a
+            // utf8 literal (NULL or unknown: UTC)
+            if (e.children.size() != 4) fail("spark_months_between() requires four arguments");
+            const int tz_at = zone_table_of(*e.children[3]);
+            Val a = gen(*e.children[0]);
+            emit(OP_TS_LOCAL_MS, a.reg, a.reg, 0, 0, VT_I64, 0, -1, unit_of(a.type));
+            Val b = gen(*e.children[1]);
+            emit(OP_TS_LOCAL_MS, b.reg, b.reg, 0, 0, VT_I64, 0, -1, unit_of(b.type));
+            Val c = cast_to(gen(*e.children[2]), DType(T_BOOL));
+            prog.need_hi = true;
+            emit(OP_MONTHS_BETWEEN, a.reg, a.reg, b.reg, c.reg, VT_F64, 0, tz_at);
+            release(b.reg);
+            release(c.reg);
+            r = Val{a.reg, DType(T_FLOAT64)};
         } else if (f == "Power") {
             Val a = cast_to(gen(*e.children[0]), DType(T_FLOAT64));
             Val b = cast_to(gen(*e.children[1]), DType(T_FLOAT64));
@@ -2378,6 +2660,7 @@ struct Compiler {
         else if (f == "Signum") r = unary_f64(M_SIGNUM);
         else if (f == "Trunc") r = unary_f64(M_TRUNC);
         else if (f == "Expm1") r = unary_f64(M_EXPM1);
+        else if (f == "Acosh") r = unary_f64(M_ACOSH);
         else fail("scalar function " + f + " is not native on device");
         if (e.type.id != T_NULL && r.type != e.type) r = cast_to(r, e.type);
         return r;
@@ -2400,7 +2683,9 @@ struct Compiler {
             case E_BINARY: return binary_cmp_or_arith(e);
             case E_SC_AND: case E_SC_OR: {
                 Val a = gen(*e.children[0]);
+                cond_depth++;
                 Val b = gen(*e.children[1]);
+                cond_depth--;
                 emit(e.kind == E_SC_AND ? OP_AND : OP_OR, a.reg, a.reg, b.reg);
                 release(b.reg);
                 return {a.reg, DType(T_BOOL)};
@@ -2445,13 +2730,16 @@ struct Compiler {
                 DType rt = infer_type(*e.children[k + 1], in);
                 if (rt.id == T_NULL && e.has_else) rt = infer_type(*e.children.back(), in);
                 // evaluate from the last branch backwards: acc = else ; acc = cond_i ? then_i : acc
+                cond_depth++;
                 Val acc = e.has_else ? cast_to(gen(*e.children.back()), rt) : literal(Literal{rt, true});
                 if (acc.type.id == T_NULL) acc.type = rt;
                 note_type(rt);
                 for (size_t pi = n_pairs; pi-- > 0;) {
                     const Expr& w = *e.children[k + 2 * pi];
                     const Expr& th = *e.children[k + 2 * pi + 1];
+                    if (pi == 0) cond_depth--;   // the first condition sees every row
                     Val cond = gen(w);
+                    if (pi == 0) cond_depth++;
                     if (e.has_case_expr) {
                         cond = cast_to(cond, base.type);
                         emit(OP_EQ, cond.reg, base.reg, cond.reg, 0, vt_of(base.type));
@@ -2461,6 +2749,7 @@ struct Compiler {
                     release(cond.reg);
                     release(tv.reg);
                 }
+                cond_depth--;
                 if (base.reg >= 0) release(base.reg);
                 return {acc.reg, rt};
             }
@@ -2478,6 +2767,13 @@ struct Compiler {
                 return {s.reg, DType(T_BOOL)};
             }
             case E_SCALAR_FN: return scalar_fn(e);
+            case E_ROW_NUM: {
+                if (!row_num_ok) fail("RowNum is only native in a projection");
+                if (cond_depth > 0) fail("RowNum is not native inside a conditional branch (CASE, coalesce, short-circuit AND / OR)");
+                const int r = alloc();
+                emit(OP_ROWNUM, r, 0, 0, 0, VT_I64);
+                return {r, DType(T_INT64)};
+            }
         }
         fail("unsupported expression kind");
     }
@@ -2521,6 +2817,19 @@ struct Compiler {
         const int fn = string_fn_of(g);
         const size_t nargs = fn <= SBF_TRANSLATE ? 3 : 1;
         if (x.children.size() != nargs) fail(g + " takes " + std::to_string(nargs) + (nargs == 1 ? " argument" : " arguments"));
+        if (fn == SBF_HEX || fn == SBF_CHR) {   // hex of an integer or of a utf8 / binary value's bytes, chr of an integer
+            Val v = gen(*x.children[0]);
+            int k = fn;
+            if (v.type.is_integer() || v.type.id == T_NULL) {
+                v = cast_to(v, DType(T_INT64));
+                if (fn == SBF_HEX) k = SBF_HEX_INT;
+            } else if (!(fn == SBF_HEX && v.type.is_varlen()))
+                fail(g + " argument of type " + v.type.str() + " is not native" + (fn == SBF_HEX ? " (integers, utf8 and binary only)" : " (integers only)"));
+            note_type(DType(T_UTF8));
+            emit(OP_SB_APPEND, b, v.reg, 0, 0, vt_of(v.type), SB_VIEW | (flags & SB_WS) | (k << 4), o | (const_idx << 8));
+            release(v.reg);
+            return;
+        }
         auto text = [&](const Expr& a) {
             Val v = gen(a);
             if (v.type.id != T_UTF8 && v.type.id != T_NULL) fail(g + " argument of type " + v.type.str() + " is not native (utf8 only)");
@@ -2616,10 +2925,11 @@ struct Compiler {
     }
 };
 
-VmProgram compile_projection(const std::vector<ExprPtr>& exprs, const Schema& input) {
+VmProgram compile_projection(const std::vector<ExprPtr>& exprs, const Schema& input, bool row_num) {
     VmProgram p;
     p.impl = std::make_shared<VmProgramImpl>();
     Compiler c(input, *p.impl);
+    c.row_num_ok = row_num;
     AURON_CHECK(exprs.size() <= VM_MAX_COLS, "too many projection expressions for one program");
     for (size_t i = 0; i < exprs.size(); i++) {
         const Expr& ex = strip_utf8_cast(*exprs[i]);
@@ -2821,7 +3131,7 @@ static void finish_offsets(Ctx& ctx, Column& c, int64_t* lens, int64_t n) {
     c.data_bytes = total;
 }
 
-std::vector<ColumnPtr> eval_projection(Ctx& ctx, const VmProgram& prog, const Batch& in, const int32_t* sel, int64_t n_out) {
+std::vector<ColumnPtr> eval_projection(Ctx& ctx, const VmProgram& prog, const Batch& in, const int32_t* sel, int64_t n_out, int64_t row_base) {
     init_pow10_tables();
     VmProgramImpl& im = *prog.impl;
     const size_t n_vis = prog.out_types.size(), n_all = n_vis + (size_t)im.n_hidden;   // hidden outputs: digest arguments
@@ -2860,6 +3170,7 @@ std::vector<ColumnPtr> eval_projection(Ctx& ctx, const VmProgram& prog, const Ba
         bind_inputs(im, in, p);
         p.sel = sel;
         p.n = n_out;
+        p.row_base = row_base;
         p.mode = 0;
         for (size_t i = 0; i < outs.size(); i++) {
             p.out_data[i] = outs[i]->data ? outs[i]->data->ptr : nullptr;

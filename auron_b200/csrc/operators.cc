@@ -92,6 +92,7 @@ std::string expr_to_string(const Expr& e) {
         case E_CONTAINS: return "Contains(" + args() + ", '" + e.lit.s + "')";
         case E_SC_AND: return "SCAnd(" + args() + ")";
         case E_SC_OR: return "SCOr(" + args() + ")";
+        case E_ROW_NUM: return "RowNum()";
     }
     return "?";
 }
@@ -287,7 +288,7 @@ ProjectExec::ProjectExec(OperatorPtr input, std::vector<ExprPtr> ex, std::vector
         out_schema.fields.push_back(f);
     }
     if (!computed.empty()) {
-        prog = compile_projection(computed, in);
+        prog = compile_projection(computed, in, true);
         has_prog = true;
     }
     children.push_back(std::move(input));
@@ -299,7 +300,8 @@ BatchPtr ProjectExec::next(Task& t) {
     auto out = std::make_shared<Batch>();
     out->num_rows = s.n;
     std::vector<ColumnPtr> computed;
-    if (has_prog) computed = eval_projection(t.ctx, prog, *s.batch, P<int32_t>(s.sel), s.n);
+    if (has_prog) computed = eval_projection(t.ctx, prog, *s.batch, P<int32_t>(s.sel), s.n, rows_out);
+    rows_out += s.n;
     for (size_t i = 0; i < exprs.size(); i++) {
         if (plain_col[i] >= 0) {
             const ColumnPtr& c = s.batch->cols[plain_col[i]];

@@ -74,6 +74,7 @@ struct ProjectExec : Operator {
     std::vector<int> prog_slot;       // index into the VM program outputs for computed exprs
     VmProgram prog;
     bool has_prog = false;
+    int64_t rows_out = 0;             // rows emitted so far: the base of RowNum
     ProjectExec(OperatorPtr input, std::vector<ExprPtr> exprs, std::vector<std::string> names, std::vector<DType> types);
     std::string describe() const override;
     BatchPtr next(Task& t) override;

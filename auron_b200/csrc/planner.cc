@@ -363,11 +363,13 @@ static const char* scalar_fn_name(int fun) {   // auron.proto ScalarFunction :21
         case 5: return "Ceil"; case 6: return "Cos"; case 8: return "Exp"; case 9: return "Floor"; case 10: return "Ln"; case 11: return "Log";
         case 12: return "Log10"; case 13: return "Log2"; case 14: return "Round"; case 15: return "Signum"; case 16: return "Sin";
         case 17: return "Sqrt"; case 18: return "Tan"; case 19: return "Trunc"; case 20: return "NullIf"; case 22: return "BitLength";
-        case 23: return "Btrim"; case 24: return "CharacterLength"; case 26: return "Concat"; case 28: return "DatePart";
-        case 32: return "Lpad"; case 33: return "Lower"; case 34: return "Ltrim"; case 37: return "OctetLength"; case 41: return "Replace";
-        case 42: return "Reverse"; case 44: return "Rpad"; case 45: return "Rtrim"; case 51: return "StartsWith";
+        case 23: return "Btrim"; case 24: return "CharacterLength"; case 25: return "Chr"; case 26: return "Concat"; case 28: return "DatePart";
+        case 29: return "DateTrunc"; case 32: return "Lpad"; case 33: return "Lower"; case 34: return "Ltrim"; case 37: return "OctetLength";
+        case 41: return "Replace"; case 42: return "Reverse"; case 44: return "Rpad"; case 45: return "Rtrim"; case 51: return "StartsWith";
         case 53: return "Substr"; case 60: return "Translate"; case 61: return "Trim"; case 62: return "Upper"; case 63: return "Coalesce";
-        case 64: return "Expm1"; case 67: return "Power"; case 69: return "IsNaN"; case 81: return "FindInSet"; case 82: return "Nvl";
+        case 64: return "Expm1"; case 65: return "Factorial"; case 66: return "Hex"; case 67: return "Power"; case 68: return "Acosh";
+        case 69: return "IsNaN"; case 80: return "Levenshtein"; case 81: return "FindInSet"; case 82: return "Nvl"; case 83: return "Nvl2";
+        case 84: return "Least"; case 85: return "Greatest"; case 86: return "MakeDate";
         default: return nullptr;
     }
 }
@@ -405,6 +407,8 @@ struct DepthGuard {
     }
     ~DepthGuard() { --g_decode_depth; }
 };
+// the partition id of the task whose plan this thread decodes (create_task): the value of SparkPartitionIdExprNode
+static thread_local uint32_t g_decode_partition_id = 0;
 
 ExprPtr decode_expr(const uint8_t* b, size_t n) {
     DepthGuard depth;
@@ -588,6 +592,15 @@ ExprPtr decode_expr(const uint8_t* b, size_t n) {
                     else if (sf == 2 && sw == 2) e->lit.s = s.bytes();
                     else s.skip(sw);
                 }
+                break;
+            case 20100:   // RowNumExprNode{}
+                e->kind = E_ROW_NUM;
+                break;
+            case 20101:   // SparkPartitionIdExprNode{}: the task's partition id, a constant of the plan (spark_partition_id.rs)
+                e->kind = E_LITERAL;
+                e->lit.type = DType(T_INT32);
+                e->lit.is_null = false;
+                e->lit.i = (int32_t)g_decode_partition_id;
                 break;
             default:
                 fail("physical expression kind #" + std::to_string(f) + " is not native on device (JVM-callback / nested-type expressions are out of scope)");
@@ -1079,6 +1092,8 @@ std::unique_ptr<Task> create_task(const uint8_t* task_def, size_t len, const aur
     t->cb = cb;
     PbReader r(task_def, len);
     uint32_t f, w;
+    const uint8_t* plan = nullptr;
+    size_t plan_len = 0;
     while (r.next(&f, &w)) {
         if (f == 1 && w == 2) {   // PartitionId{stage_id=2, partition_id=4, task_id=5}
             const uint8_t* sb;
@@ -1092,12 +1107,12 @@ std::unique_ptr<Task> create_task(const uint8_t* task_def, size_t len, const aur
                 else if (sf == 5 && sw == 0) t->task_id = s.varint();
                 else s.skip(sw);
             }
-        } else if (f == 2 && w == 2) {
-            const uint8_t* sb;
-            size_t sn;
-            r.bytes_view(&sb, &sn);
-            t->root = decode_plan(*t, sb, sn);
-        } else r.skip(w);
+        } else if (f == 2 && w == 2) r.bytes_view(&plan, &plan_len);   // decoded once the partition id is known
+        else r.skip(w);
+    }
+    if (plan) {
+        g_decode_partition_id = t->partition_id;
+        t->root = decode_plan(*t, plan, plan_len);
     }
     AURON_CHECK(t->root != nullptr, "TaskDefinition without a plan");
     return t;

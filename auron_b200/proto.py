@@ -158,9 +158,10 @@ def in_list(e: bytes, items: list[bytes], negated: bool = False) -> bytes:
 
 
 SCALAR_FN = {"Abs": 0, "Ascii": 4, "Ceil": 5, "Exp": 8, "Floor": 9, "Ln": 10, "Log10": 12, "Log2": 13, "Signum": 15, "Sqrt": 17,
-             "NullIf": 20, "BitLength": 22, "CharacterLength": 24, "DatePart": 28, "Lpad": 32, "Lower": 33, "Ltrim": 34, "OctetLength": 37,
-             "Replace": 41, "Reverse": 42, "Rpad": 44, "Rtrim": 45, "StartsWith": 51, "Substr": 53, "Translate": 60, "Trim": 61,
-             "Upper": 62, "Coalesce": 63, "Power": 67, "IsNaN": 69, "FindInSet": 81, "AuronExtFunctions": 10000}
+             "NullIf": 20, "BitLength": 22, "CharacterLength": 24, "Chr": 25, "DatePart": 28, "DateTrunc": 29, "Lpad": 32, "Lower": 33,
+             "Ltrim": 34, "OctetLength": 37, "Replace": 41, "Reverse": 42, "Rpad": 44, "Rtrim": 45, "StartsWith": 51, "Substr": 53,
+             "Translate": 60, "Trim": 61, "Upper": 62, "Coalesce": 63, "Factorial": 65, "Hex": 66, "Power": 67, "Acosh": 68, "IsNaN": 69,
+             "Levenshtein": 80, "FindInSet": 81, "Nvl2": 83, "Least": 84, "Greatest": 85, "MakeDate": 86, "AuronExtFunctions": 10000}
 
 
 def scalar_fn(name: str, args: list[bytes], return_type: pa.DataType) -> bytes:
@@ -191,6 +192,16 @@ def ends_with(e: bytes, suffix: str) -> bytes:
 
 def contains(e: bytes, infix: str) -> bytes:
     return f_bytes(20002, f_bytes(1, e) + f_str(2, infix))
+
+
+def row_num() -> bytes:
+    """PhysicalExprNode{row_num_expr} (NativeConverters.scala StubExpr("RowNum"))"""
+    return f_bytes(20100, b"")
+
+
+def spark_partition_id() -> bytes:
+    """PhysicalExprNode{spark_partition_id_expr}"""
+    return f_bytes(20101, b"")
 
 
 AGG_FN = {"MIN": 0, "MAX": 1, "SUM": 2, "AVG": 3, "COUNT": 4, "FIRST": 7, "FIRST_IGNORES_NULL": 8}

@@ -2,7 +2,7 @@
 time per launch site from the library's CUDA-event timers (AURON_PROFILE=1).  These are the operator-level numbers the
 north star asks for next to the config-2 bench line; they are not bench.py lines.
 
-    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [window]
+    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [scalar] [window]
 
   join     cfg 3: store_sales (N rows: ss_sold_date_sk int32, ss_item_sk int32, ss_quantity int32) JOIN date_dim (73,049 rows:
            d_date_sk int32, d_year int32) on the date key, inner, build = date_dim
@@ -15,6 +15,8 @@ north star asks for next to the config-2 bench line; they are not bench.py lines
   filter_project  cfg 1 shape on the expression VM: Project[a + 1, substr(s, 1, 4), CAST(d * 3 AS decimal(38, 2))] <-
            Filter[a > 100000 AND s LIKE 'a%'] over N rows (a int64 1 % NULL, s utf8 4-24 B, d int64), + COUNT / SUM so that one
            row leaves the GPU; the decimal output runs the 128-bit variant of vm_kernel
+  scalar   months_between(t1, t2, true, 'America/New_York'), date_trunc('MONTH', t1) and greatest(g0, ..., g7) over N rows of
+           (t1, t2 timestamp(us) in 1906-2096, g0..g7 int64 with 5 % NULL), each projection feeding a COUNT
   window   WindowExec over N pre-sorted rows (p int32, ~1,000 rows per partition; o int64; v decimal(17,2), 5 % NULL; s utf8 8-24 B)
            in device batches of 16M rows, so the running state carries across batch edges: ROW_NUMBER, RANK, SUM(v), AVG(v), MAX(s),
            COUNT(v) partitioned by p ordered by o, + COUNT / SUM so that one row leaves the GPU
@@ -241,6 +243,30 @@ if "filter_project" in which:
     plan = P.agg(proj, [], [], [P.agg_expr("COUNT", [P.col("s4")], pa.int64()), P.agg_expr("SUM", [P.col("a1")], pa.int64())], ["c", "x"], ["PARTIAL"] * 2)
     run(plan, f"cfg1 shape Filter -> Project (decimal output) over {N} rows", N, steps=6)
     runtime.drop_device_resource("fp")
+
+if "scalar" in which:
+    import subprocess
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"== scalar leg on: {gpu}")
+    TS = pa.timestamp("us")
+    names = ["t1", "t2"] + [f"g{k}" for k in range(8)]
+    for start in range(0, N, CHUNK):
+        n = min(CHUNK, N - start)
+        ts = [pa.array(rng.integers(-2 * 10**15, 4 * 10**15, n)).cast(TS) for _ in range(2)]   # 1906 .. 2096
+        gs = [pa.array(rng.integers(-2**62, 2**62, n), mask=rng.random(n) < 0.05) for _ in range(8)]
+        runtime.put_device_batch("sc", pa.record_batch(ts + gs, names=names))
+    sch = pa.schema([(k, TS) for k in names[:2]] + [(k, pa.int64()) for k in names[2:]])
+    cases = [("months_between(t1, t2, true, 'America/New_York')",
+              P.scalar_fn("Spark_MonthsBetween", [P.col("t1"), P.col("t2"), P.lit(True, pa.bool_()), P.lit("America/New_York", pa.string())], pa.float64()),
+              pa.float64(), 2 * 8 * N + 8 * N),
+             ("date_trunc('MONTH', t1)", P.scalar_fn("DateTrunc", [P.lit("MONTH", pa.string()), P.col("t1")], TS), TS, 8 * N + 8 * N),
+             ("greatest(g0, ..., g7)", P.scalar_fn("Greatest", [P.col(f"g{k}") for k in range(8)], pa.int64()), pa.int64(), 8 * 8 * N + 8 * N)]
+    for label, expr, t, alg in cases:   # algorithmic bytes: the input columns once + the output once (validity bits left out)
+        proj = P.projection(P.ffi_reader(sch, "sc"), [expr], ["x"], [t])
+        plan = P.agg(proj, [], [], [P.agg_expr("COUNT", [P.col("x")], pa.int64())], ["c"], ["PARTIAL"])
+        run(plan, f"{label} over {N} rows", N, alg={"expr_vm": alg})
+    runtime.drop_device_resource("sc")
 
 if "window" in which:
     import subprocess
