@@ -202,6 +202,26 @@ int auron_b200_digest_hex(int32_t alg, const uint8_t* bytes, int64_t len, char* 
     API_GUARD_END(-1)
 }
 
+int auron_b200_float_to_text(int32_t bits, uint64_t value, char* out) {
+    API_GUARD_BEGIN
+    if (!out || (bits != 32 && bits != 64) || (bits == 32 && value >> 32)) {
+        g_last_error = "float_to_text: bits must be 32 or 64, the value a bit pattern of that width, out non-null";
+        return -1;
+    }
+    return float_to_text_host(bits, value, out);
+    API_GUARD_END(-1)
+}
+
+int auron_b200_text_to_float(int32_t bits, const uint8_t* text, int64_t len, uint64_t* value) {
+    API_GUARD_BEGIN
+    if (!value || (bits != 32 && bits != 64) || len < 0 || len > INT32_MAX || (len > 0 && !text)) {
+        g_last_error = "text_to_float: bits must be 32 or 64, len in 0..2^31-1, text and value non-null";
+        return -1;
+    }
+    return text_to_float_host(bits, text, (int32_t)len, value) ? 1 : 0;
+    API_GUARD_END(-1)
+}
+
 // ---- device residency
 static std::map<int, std::unique_ptr<Ctx>>& util_ctxs() {
     static std::map<int, std::unique_ptr<Ctx>> m;

@@ -26,6 +26,7 @@
 
 #include "device_utils.cuh"
 #include "expr.h"
+#include "float_text.cuh"
 #include "kernels.h"
 #include "tzdb.h"
 
@@ -99,8 +100,8 @@ struct VmParams {
 };
 
 // 10^k as 128-bit, k = 0..38
-__constant__ uint64_t c_pow10_lo[39];
-__constant__ int64_t c_pow10_hi[39];
+static __constant__ uint64_t c_pow10_lo[39];
+static __constant__ int64_t c_pow10_hi[39];
 static void init_pow10_tables() {
     static bool done = false;
     if (done) return;
@@ -351,7 +352,7 @@ __device__ inline int64_t ts_to_local_ms(int64_t v, int unit, const uint8_t* tz)
 // later).  false when there is none.  Interval k (offset o, UTC [trans[k - 1], trans[k])) holds the local times
 // [trans[k - 1] + o, trans[k] + o), so its first minute is found without walking; offsets lie within +-26 h, so only the intervals
 // that cover [local_s - 26 h, local_s + 50 h] can hold the answer.  Out of line: inlined, it makes vm_kernel<true> spill.
-__device__ __noinline__ bool local_to_utc_s(const uint8_t* tz, int64_t local_s, int64_t* out) {
+static __device__ __noinline__ bool local_to_utc_s(const uint8_t* tz, int64_t local_s, int64_t* out) {
     const int64_t n = *(const int64_t*)tz;
     const int64_t* trans = (const int64_t*)tz + 1;
     const int64_t k0 = tz_interval(tz, local_s - 93600), k1 = tz_interval(tz, local_s + 180000);
@@ -770,8 +771,10 @@ __device__ inline bool vm_cast(const VmParams& p, int st, int dt, int sscale, in
 
 // ------------------------------------------------------------------------------------------ the VM kernel
 // ---- CAST(x AS STRING) of a projection output (TryCastExpr -> arrow cast; bool: cast.rs:104-112, decimal: cast.rs:660-690):
-// format `kind` value into buf (>= 24 bytes), returns the length.  kind: 0 bool, 1 integer, 2 date32, 3 decimal (scale)
-enum FmtKind : int { FMT_BOOL = 0, FMT_INT = 1, FMT_DATE = 2, FMT_DEC = 3 };
+// format `kind` value into buf (>= 42 bytes), returns the length.  kind: 0 bool, 1 integer, 2 date32, 3 decimal (scale), 4 float32,
+// 5 float64 (Java's Float / Double.toString, float_text.cuh).  Floats and decimal(p > 18) run in vm_kernel<true, true> only (the
+// compiler sets need_text for them).
+enum FmtKind : int { FMT_BOOL = 0, FMT_INT = 1, FMT_DATE = 2, FMT_DEC = 3, FMT_F32 = 4, FMT_F64 = 5 };
 __device__ inline int fmt_u64(uint64_t v, char* end) {   // writes digits backwards, returns count
     int n = 0;
     do {
@@ -781,7 +784,41 @@ __device__ inline int fmt_u64(uint64_t v, char* end) {   // writes digits backwa
     } while (v);
     return n;
 }
-__device__ inline int fmt_value(int kind, int scale, uint64_t lo, char* buf) {
+// the unscaled i128 {lo, hi} at `scale`: a '-', the integer part (at least "0"), '.', `scale` fractional digits (cast.rs:660-690)
+__device__ __forceinline__ int fmt_decimal(uint64_t lo, int64_t hi, int scale, char* buf) {
+    char tmp[40];
+    char* end = tmp + 40;
+    const bool neg = hi < 0;
+    const i128 mag = i128_abs({lo, hi});
+    uint64_t low;
+    const i128 top = u128_divmod_u64(mag, 10000000000000000000ull, &low);   // |v| <= 2^127: top < 2^64
+    int n = fmt_u64(low, end);
+    if (top.lo) {
+        while (n < 19) *(end - ++n) = '0';
+        n += fmt_u64(top.lo, end - n);
+    }
+    const char* digits = end - n;
+    int k = 0;
+    if (neg) buf[k++] = '-';
+    if (scale <= 0) {
+        for (int i = 0; i < n; i++) buf[k++] = digits[i];
+    } else if (n > scale) {
+        for (int i = 0; i < n - scale; i++) buf[k++] = digits[i];
+        buf[k++] = '.';
+        for (int i = n - scale; i < n; i++) buf[k++] = digits[i];
+    } else {
+        buf[k++] = '0';
+        buf[k++] = '.';
+        for (int i = n; i < scale; i++) buf[k++] = '0';
+        for (int i = 0; i < n; i++) buf[k++] = digits[i];
+    }
+    return k;
+}
+template <bool TEXT>
+__device__ inline int fmt_value(int kind, int scale, uint64_t lo, int64_t hi, char* buf) {
+    if (TEXT && kind == FMT_DEC) return fmt_decimal(lo, hi, scale, buf);
+    if (TEXT && kind >= FMT_F32) return ft_float_to_text(kind == FMT_F32 ? 32 : 64, lo, buf);
+    // bool, integers, dates and decimal(p <= 18): the unscaled value fits lo
     char tmp[24];
     char* end = tmp + 24;
     int n = 0;
@@ -865,6 +902,28 @@ struct SView {
     }
 };
 __device__ __forceinline__ SView sview(const VmParams& p, int64_t h, uint64_t x) { return {str_ptr(p, h, x), str_len(x), (int)((h >> 8) & 0xff)}; }
+// CAST(utf8 AS BOOLEAN), Spark's StringUtils.isTrueString / isFalseString: ASCII whitespace and control characters trimmed at
+// both ends, ASCII case ignored; t true y yes 1 -> true, f false n no 0 -> false, anything else NULL
+__device__ inline bool str_to_bool(const SView& s, uint64_t* out) {
+    int32_t a = 0, e = s.n;
+    while (a < e && (s.p[a] <= ' ' || s.p[a] == 0x7f)) a++;
+    while (e > a && (s.p[e - 1] <= ' ' || s.p[e - 1] == 0x7f)) e--;
+    const uint8_t* t = s.p + a;
+    const int32_t n = e - a;
+    if (ft_word(t, n, "t", true) || ft_word(t, n, "true", true) || ft_word(t, n, "y", true) || ft_word(t, n, "yes", true) || ft_word(t, n, "1", true))
+        *out = 1;
+    else if (ft_word(t, n, "f", true) || ft_word(t, n, "false", true) || ft_word(t, n, "n", true) || ft_word(t, n, "no", true) || ft_word(t, n, "0", true))
+        *out = 0;
+    else return false;
+    return true;
+}
+// CAST(utf8 AS FLOAT / DOUBLE / BOOLEAN) of the view {lo, hi}; returns the validity, the value in lo
+static __device__ __noinline__ bool str_to_float_or_bool(const VmParams& p, int dt, uint64_t& lo, int64_t& hi) {
+    const SView s = sview(p, hi, lo);
+    hi = 0;
+    if (dt == VT_BOOL) return str_to_bool(s, &lo);
+    return ft_text_to_float(dt == VT_F32 ? 32 : 64, s.p, s.n, s.xf != 0, &lo);
+}
 // unsigned byte order, the shorter prefix first
 __device__ inline int sv_cmp(const SView& a, const SView& b) {
     if (a.xf == 0 && b.xf == 0) return str_cmp(a.p, a.n, b.p, b.n);
@@ -1063,7 +1122,9 @@ __device__ inline int64_t sb_fn_piece(int fn, const SView& s, const SView& x, co
     }
 }
 
-template <bool HI>
+// TEXT (implies HI): the program formats decimals or floats as text or parses floats or booleans from it.  That code runs in
+// its own instantiation: calls into it cost the other programs of vm_kernel<true> registers and stack.
+template <bool HI, bool TEXT = false>
 __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
     extern __shared__ __align__(16) uint64_t vm_smem[];
     uint64_t* LO = vm_smem;
@@ -1272,7 +1333,10 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                     int64_t hi = HI ? RHI(ins.a) : 0;
                     int dt = ins.aux & 0xff, sscale = (ins.aux >> 8) & 0xff;
                     int dprec = (int8_t)((ins.aux2 >> 8) & 0xff), dscale = (int8_t)(ins.aux2 & 0xff);
-                    if (v) v = vm_cast(p, t, dt, sscale, dprec, dscale, lo, hi);
+                    if (v) {   // utf8 -> float / bool only in vm_kernel<true, true> (the compiler sets need_text for them)
+                        if (TEXT && t == VT_STR && (dt == VT_F32 || dt == VT_F64 || dt == VT_BOOL)) v = str_to_float_or_bool(p, dt, lo, hi);
+                        else v = vm_cast(p, t, dt, sscale, dprec, dscale, lo, hi);
+                    }
                     RLO(ins.dst) = v ? lo : 0;
                     if (HI) RHI(ins.dst) = v ? hi : 0;
                     SETV(ins.dst, v);
@@ -1647,7 +1711,7 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                 case OP_FMT_OUT: {   // CAST(value AS STRING) straight into a utf8 output column (both passes format the value)
                     const int o = ins.aux;
                     bool v = active && VALID(ins.a);
-                    int len = v ? fmt_value((ins.aux2 >> 8) & 0xff, ins.aux2 & 0xff, RLO(ins.a), buf) : 0;
+                    int len = v ? fmt_value<TEXT>((ins.aux2 >> 8) & 0xff, ins.aux2 & 0xff, RLO(ins.a), TEXT ? RHI(ins.a) : 0, buf) : 0;
                     if (p.mode == 0) {
                         if (active) p.out_lens[o][i] = len;
                         uint32_t w = __ballot_sync(FULL_MASK, v);
@@ -1711,7 +1775,7 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
                         int32_t len;
                         int xf = 0;
                         if (kind == SB_FMT) {
-                            len = fmt_value((ins.aux2 >> 8) & 0xff, ins.aux2 & 0xff, x, buf);
+                            len = fmt_value<TEXT>((ins.aux2 >> 8) & 0xff, ins.aux2 & 0xff, x, TEXT ? RHI(ins.a) : 0, buf);
                             s = (const uint8_t*)buf;
                         } else {
                             const int64_t h = RHI(ins.a);
@@ -1750,6 +1814,20 @@ __global__ void __launch_bounds__(VM_THREADS) vm_kernel(VmParams p) {
 #undef SETV
 }
 
+// vm_kernel<true, true> is compiled in a translation unit of its own (k_expr_text.cu, which includes this file): its out-of-line
+// calls into the text casts, in one module with the other instantiations, cost vm_kernel<true> spills.
+void launch_vm_text(unsigned grid, size_t smem, cudaStream_t stream, const VmParams& p);
+#ifdef AURON_VM_TEXT_TU
+void launch_vm_text(unsigned grid, size_t smem, cudaStream_t stream, const VmParams& p) {
+    static bool attr = false;
+    init_pow10_tables();   // this module's copy
+    if (!attr) {
+        CUDA_OK(cudaFuncSetAttribute(vm_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 2 * VM_NREG * VM_THREADS * 8 + 1024 * 16));
+        attr = true;
+    }
+    vm_kernel<true, true><<<grid, VM_THREADS, smem, stream>>>(p);
+}
+#else
 // ------------------------------------------------------------------------------------------ conjunctive compare fast path
 // The overwhelmingly common filter shape (TPC-DS: BETWEEN, =, <, IS NOT NULL on fixed-width columns) is a conjunction of
 // `column <op> literal` terms.  Those skip the interpreter: every thread loads each referenced column once into
@@ -1978,6 +2056,7 @@ struct VmProgramImpl {
     std::vector<Digest> digests;
     int n_hidden = 0;
     bool need_hi = false;
+    bool need_text = false;   // float / decimal text casts: vm_kernel<true, true>
     // device copies (uploaded lazily per ctx stream; programs are immutable after compile)
     Buf d_code, d_consts, d_pool;
 };
@@ -2076,12 +2155,17 @@ static int fmt_kind_of(const DType& st, int* scale) {
     if (st.id == T_BOOL) return FMT_BOOL;
     if (st.is_integer()) return FMT_INT;
     if (st.id == T_DATE32) return FMT_DATE;
-    if (st.id == T_DECIMAL128 && st.precision <= 18 && st.scale >= 0 && st.scale <= 18) {
+    if (st.id == T_DECIMAL128 && st.scale >= 0 && st.scale <= 38) {
         *scale = st.scale;
         return FMT_DEC;
     }
+    if (st.id == T_FLOAT32) return FMT_F32;
+    if (st.id == T_FLOAT64) return FMT_F64;
     return -1;
 }
+
+// the kinds fmt_value formats in vm_kernel<true, true> only
+static bool needs_text(int kind, const DType& st) { return kind == FMT_F32 || kind == FMT_F64 || (kind == FMT_DEC && st.precision > 18); }
 
 static bool is_cmp_op(const std::string& op) {
     return op == "Eq" || op == "NotEq" || op == "Lt" || op == "LtEq" || op == "Gt" || op == "GtEq" || op == "IsDistinctFrom" || op == "IsNotDistinctFrom";
@@ -2216,7 +2300,8 @@ struct Compiler {
         emit(OP_CONST, r, 0, 0, 0, 0, 0, ci);
         return {r, l.type};
     }
-    Val cast_to(Val v, const DType& to) {
+    // explicit: a CAST / TRY_CAST of the plan, not a coercion the compiler inserts (only those parse text into floats / bools)
+    Val cast_to(Val v, const DType& to, bool explicit_cast = false) {
         if (v.type == to) return v;
         if (v.type.id == T_NULL) {   // typed NULL
             emit(OP_CONST, v.reg, 0, 0, 0, 0, 0, add_const(0, to.is_varlen() ? VM_POOL_BUF : 0, false));
@@ -2231,6 +2316,10 @@ struct Compiler {
         if ((st == VT_F32 || st == VT_F64) && dt != VT_STR) ok = true;
         if (st == VT_DEC && dt != VT_STR && dt != VT_BOOL) ok = true;
         if (st == VT_STR && ((dt >= VT_I8 && dt <= VT_I64 && to.is_integer()) || date_target || dt == VT_DEC)) ok = true;
+        if (explicit_cast && v.type.id == T_UTF8 && (dt == VT_F32 || dt == VT_F64 || dt == VT_BOOL)) {   // Spark's parsers (float_text.cuh, str_to_bool)
+            ok = true;
+            prog.need_hi = prog.need_text = true;   // they run in vm_kernel<true, true> only
+        }
         if (st == VT_STR && dt == VT_STR) return {v.reg, to};
         // same physical representation (date32 <-> int32 etc.) are not native casts in the reference
         if ((v.type.id == T_DATE32 || to.id == T_DATE32 || v.type.id == T_TIMESTAMP || to.id == T_TIMESTAMP || v.type.id == T_DATE64 || to.id == T_DATE64) &&
@@ -2706,7 +2795,7 @@ struct Compiler {
                 emit(OP_NEG, a.reg, a.reg, 0, 0, vt_of(a.type));
                 return a;
             }
-            case E_CAST: case E_TRY_CAST: return cast_to(gen(*e.children[0]), e.type);
+            case E_CAST: case E_TRY_CAST: return cast_to(gen(*e.children[0]), e.type, true);
             case E_IN_LIST: {
                 Val x = gen(*e.children[0]);
                 note_type(x.type);
@@ -2798,11 +2887,13 @@ struct Compiler {
         if ((x.kind == E_CAST || x.kind == E_TRY_CAST) && x.type.id == T_UTF8) {
             const DType st = infer_type(*x.children[0], in);
             kind = fmt_kind_of(st, &scale);
+            if (kind == FMT_F32 || kind == FMT_F64) kind = -1;   // float pieces are not built yet
             if (kind < 0 && st.id != T_UTF8 && st.id != T_NULL) fail(f + ": CAST " + st.str() + " -> utf8 is not native on device");
         }
         Val v = kind >= 0 ? gen(*x.children[0]) : gen(x);
         if (kind >= 0) {
             note_type(v.type);
+            if (needs_text(kind, v.type)) prog.need_text = true;
             emit(OP_SB_APPEND, b, v.reg, 0, 0, vt_of(v.type), SB_FMT | flags, o | (const_idx << 8), (kind << 8) | scale);
         } else {
             if (v.type.id != T_UTF8 && v.type.id != T_NULL) fail(f + " argument of type " + v.type.str() + " is not native (utf8 pieces only)");
@@ -2910,6 +3001,7 @@ struct Compiler {
                 Val v = gen(*ex.children[0]);
                 note_type(v.type);
                 note_type(ex.type);
+                if (needs_text(kind, v.type)) prog.need_hi = prog.need_text = true;   // fmt_value formats them in vm_kernel<true, true> only
                 emit(OP_FMT_OUT, 0, v.reg, 0, 0, vt_of(v.type), 0, o, (kind << 8) | scale);
                 release(v.reg);
                 return ex.type;
@@ -3109,7 +3201,8 @@ static void launch_vm(Ctx& ctx, const VmProgramImpl& im, const VmParams& p) {
     int per_sm = im.need_hi ? 3 : 6;
     unsigned grid = (unsigned)std::max<int64_t>(1, std::min<int64_t>(blocks, (int64_t)ctx.sm_count * per_sm));
     ProfScope ps(ctx, "expr_vm");
-    if (im.need_hi) vm_kernel<true><<<grid, VM_THREADS, smem, ctx.stream>>>(p);
+    if (im.need_text) launch_vm_text(grid, smem, ctx.stream, p);
+    else if (im.need_hi) vm_kernel<true><<<grid, VM_THREADS, smem, ctx.stream>>>(p);
     else vm_kernel<false><<<grid, VM_THREADS, smem, ctx.stream>>>(p);
     LAUNCH_CHECK(ctx);
 }
@@ -3268,5 +3361,9 @@ Buf eval_predicate(Ctx& ctx, const VmProgram& prog, const Batch& in, int64_t n_r
     launch_vm(ctx, im, p);
     return mask;
 }
+
+int float_to_text_host(int bits, uint64_t value, char* out) { return ft_float_to_text(bits, value, out); }
+bool text_to_float_host(int bits, const uint8_t* text, int32_t len, uint64_t* value) { return ft_text_to_float(bits, text, len, false, value); }
+#endif
 
 }  // namespace auron

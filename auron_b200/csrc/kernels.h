@@ -49,6 +49,11 @@ void digest_hex(Ctx& ctx, int alg, const int32_t* in_off, const uint8_t* in_data
 // the same computation on the CPU: writes digest_hex_width(alg) characters to out, returns that width or -1
 int digest_hex_host(int alg, const uint8_t* bytes, int64_t len, char* out);
 
+// ----------------------------------------------------------------------------- k_expr.cu: the float <-> text casts on the CPU
+// (float_text.cuh, the code the device runs).  bits: 32 or 64; values are bit patterns.
+int float_to_text_host(int bits, uint64_t value, char* out);   // Java's Float / Double.toString into out (>= 24 bytes); the length
+bool text_to_float_host(int bits, const uint8_t* text, int32_t len, uint64_t* value);   // Spark's CAST; false: NULL
+
 // ----------------------------------------------------------------------------- k_rowkeys.cu
 // Row-key view over key columns for hash aggregation / joins (general path)
 struct KeyColDesc {

@@ -158,6 +158,14 @@ int auron_b200_tz_offset(const char* zone, int64_t utc_second, int32_t* offset);
  * or 512.  Writes 32 / 56 / 64 / 96 / 128 characters to `out` (no terminator) and returns that count, or -1 for an unknown `alg`.
  * Host only: usable without a GPU. */
 int auron_b200_digest_hex(int32_t alg, const uint8_t* bytes, int64_t len, char* out);
+/* CAST(float AS STRING) of the float32 (bits 32) or float64 (bits 64) with bit pattern `value`, by the code the device's expression
+ * VM runs: Java's Float / Double.toString as specified since JDK 19.  Writes at most 24 characters to `out` (no terminator) and
+ * returns that count, or -1 for a bad argument.  Host only: usable without a GPU. */
+int auron_b200_float_to_text(int32_t bits, uint64_t value, char* out);
+/* CAST(text AS FLOAT / DOUBLE) of `len` bytes, Spark's non-ANSI semantics, by the code the device runs: writes the float32 (bits 32)
+ * or float64 (bits 64) bit pattern to *value and returns 1, returns 0 where the cast gives NULL, -1 for a bad argument.
+ * Host only: usable without a GPU. */
+int auron_b200_text_to_float(int32_t bits, const uint8_t* text, int64_t len, uint64_t* value);
 /* What the engine's Parquet metadata reader sees in the local file `path`, as JSON: footer (schema elements, row groups, column
  * chunks with codec / sizes / offsets / statistics as hex) plus, per chunk, the walk of its page headers (page counts, value
  * counts, encodings; SNAPPY bodies are run through the engine's block decoder).  The reference reads the same structures with

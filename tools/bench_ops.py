@@ -2,7 +2,7 @@
 time per launch site from the library's CUDA-event timers (AURON_PROFILE=1).  These are the operator-level numbers the
 north star asks for next to the config-2 bench line; they are not bench.py lines.
 
-    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [scalar] [window]
+    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [scalar] [casts] [window]
 
   join     cfg 3: store_sales (N rows: ss_sold_date_sk int32, ss_item_sk int32, ss_quantity int32) JOIN date_dim (73,049 rows:
            d_date_sk int32, d_year int32) on the date key, inner, build = date_dim
@@ -17,6 +17,12 @@ north star asks for next to the config-2 bench line; they are not bench.py lines
            row leaves the GPU; the decimal output runs the 128-bit variant of vm_kernel
   scalar   months_between(t1, t2, true, 'America/New_York'), date_trunc('MONTH', t1) and greatest(g0, ..., g7) over N rows of
            (t1, t2 timestamp(us) in 1906-2096, g0..g7 int64 with 5 % NULL), each projection feeding a COUNT
+  casts    CAST(f64 AS STRING), CAST(f32 AS STRING) over N random bit patterns; CAST(s AS DOUBLE) over three text shapes -- short
+           ("123.45"), 17 significant digits ("0.12345678901234567") and 55-digit exact halfway points between neighbouring doubles,
+           which take the exact fallback -- and CAST(s AS BOOLEAN), each over N rows and feeding a COUNT.  Reports expr_vm device time,
+           rows/s and algorithmic GB/s (text bytes + offsets and fixed-width values, input once + output once; the formatted text's bytes
+           are counted in an untimed pass).  Then the Filter -> Project leg three times, each time followed by the same leg of the
+           built checkout at $OPS_PARENT when that is set
   window   WindowExec over N pre-sorted rows (p int32, ~1,000 rows per partition; o int64; v decimal(17,2), 5 % NULL; s utf8 8-24 B)
            in device batches of 16M rows, so the running state carries across batch edges: ROW_NUMBER, RANK, SUM(v), AVG(v), MAX(s),
            COUNT(v) partitioned by p ordered by o, + COUNT / SUM so that one row leaves the GPU
@@ -224,7 +230,7 @@ if "strings" in which:
                       f"{calls / t / 1e9:.2f} G compression calls/s ({calls / N:.2f} per row)")
         runtime.drop_device_resource(f"str{mean}")
 
-if "filter_project" in which:
+def filter_project_leg():
     pool = rng.integers(97, 123, 1 << 20, dtype=np.uint8)
     for start in range(0, N, CHUNK):
         n = min(CHUNK, N - start)
@@ -241,8 +247,94 @@ if "filter_project" in which:
                               P.cast(P.binary("Multiply", P.col("d"), P.lit(3, pa.int64())), pa.decimal128(38, 2))],
                         ["a1", "s4", "dd"], [pa.int64(), pa.string(), pa.decimal128(38, 2)])
     plan = P.agg(proj, [], [], [P.agg_expr("COUNT", [P.col("s4")], pa.int64()), P.agg_expr("SUM", [P.col("a1")], pa.int64())], ["c", "x"], ["PARTIAL"] * 2)
-    run(plan, f"cfg1 shape Filter -> Project (decimal output) over {N} rows", N, steps=6)
+    kern = run(plan, f"cfg1 shape Filter -> Project (decimal output) over {N} rows", N, steps=6)
     runtime.drop_device_resource("fp")
+    return kern
+
+
+if "filter_project" in which:
+    filter_project_leg()
+
+if "casts" in which:
+    import re
+    import subprocess
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"== casts leg on: {gpu}")
+    U = pa.string()
+    SUB = 8_000_000   # rows per batch of the text shapes: 8M rows x 55 B stay far below 2 GiB
+
+    def text_array(mat):   # the fixed-width rows of a uint8 matrix as utf8
+        n, w = mat.shape
+        return pa.Array.from_buffers(U, n, [None, pa.py_buffer(np.arange(n + 1, dtype=np.int32) * w), pa.py_buffer(np.ascontiguousarray(mat).tobytes())])
+
+    def digits(n, w):
+        return rng.integers(48, 58, (n, w), dtype=np.uint8)
+
+    # 55-digit exact halfway points between neighbouring doubles in [1, 2): (2m + 1) / 2^53 = (2m + 1) * 5^53 / 10^53
+    half_pool = np.frombuffer(b"".join((lambda t: t[:1] + b"." + t[1:])(str((2 * int(m) + 1) * 5**53).encode())
+                                       for m in rng.integers(2**52, 2**53, 1 << 16, dtype=np.int64)), dtype=np.uint8).reshape(-1, 55)
+    bool_pool = np.frombuffer(b"true false    t    f  yes   no    1    0maybe", dtype=np.uint8).reshape(-1, 5)
+
+    def shape(kind, n):
+        if kind == "short":    # ddd.dd
+            m = digits(n, 6)
+            m[:, 3] = ord(".")
+            return m
+        if kind == "repr17":   # 0. and 17 significant digits
+            m = digits(n, 19)
+            m[:, 0], m[:, 1] = ord("0"), ord(".")
+            m[:, 2] = rng.integers(49, 58, n, dtype=np.uint8)
+            return m
+        if kind == "halfway":
+            return half_pool[rng.integers(0, len(half_pool), n)]
+        return bool_pool[rng.integers(0, len(bool_pool), n)]
+
+    for kind in ("short", "repr17", "halfway", "bool"):
+        for start in range(0, N, SUB):
+            runtime.put_device_batch(f"tx_{kind}", pa.record_batch([text_array(shape(kind, min(SUB, N - start)))], names=["s"]))
+    for start in range(0, N, CHUNK):
+        n = min(CHUNK, N - start)
+        d = (rng.integers(0, 2**63, n, dtype=np.int64).view(np.uint64) | (rng.integers(0, 2, n, dtype=np.uint64) << np.uint64(63))).view(np.float64)
+        g = rng.integers(0, 2**32, n, dtype=np.uint64).astype(np.uint32).view(np.float32)
+        runtime.put_device_batch("fl", pa.record_batch([pa.array(d), pa.array(g)], names=["d", "g"]))
+    fl_sch = pa.schema([("d", pa.float64()), ("g", pa.float32())])
+    tx_sch = pa.schema([("s", U)])
+
+    def text_bytes(col):   # untimed: the output text bytes of CAST(col AS STRING)
+        proj = P.projection(P.ffi_reader(fl_sch, "fl"), [P.cast(P.col(col), U)], ["x"], [U])
+        proj = P.projection(proj, [P.scalar_fn("OctetLength", [P.col("x")], pa.int32())], ["l"], [pa.int32()])
+        plan = P.agg(proj, [], [], [P.agg_expr("SUM", [P.col("l")], pa.int64())], ["b"], ["PARTIAL"])
+        with runtime.Task(P.task_definition(plan)) as task:
+            return sum(b.column(0).to_pylist()[0] or 0 for b in task)
+
+    # label, resource, schema, expression, result type, algorithmic bytes (input once + output once)
+    cases = []
+    for col, t, w in (("d", pa.float64(), 8), ("g", pa.float32(), 4)):
+        cases.append((f"CAST({col} {t} AS STRING)", "fl", fl_sch, P.cast(P.col(col), U), U, w * N + text_bytes(col) + 4 * (N + 1)))
+    for kind, width in (("short", 6), ("repr17", 19), ("halfway", 55)):
+        cases.append((f"CAST(s AS DOUBLE), {kind} text ({width} B)", f"tx_{kind}", tx_sch, P.cast(P.col("s"), pa.float64()), pa.float64(),
+                      (width + 4) * N + 8 * N))
+    cases.append(("CAST(s AS BOOLEAN), 5 B text", "tx_bool", tx_sch, P.cast(P.col("s"), pa.bool_()), pa.bool_(), 9 * N + N // 8))
+    for label, res, sch, expr, t, alg in cases:
+        proj = P.projection(P.ffi_reader(sch, res), [expr], ["x"], [t])
+        plan = P.agg(proj, [], [], [P.agg_expr("COUNT", [P.col("x")], pa.int64())], ["c"], ["PARTIAL"])
+        us = run(plan, f"{label} over {N} rows", N, steps=3, alg={"expr_vm": alg})
+        if us.get("expr_vm"):
+            sec = us["expr_vm"] * 1e-6
+            print(f"     expr_vm: {N / sec / 1e9:.2f} G rows/s, {alg / sec / 1e9:.0f} GB/s algorithmic")
+    for r in ("fl", "tx_short", "tx_repr17", "tx_halfway", "tx_bool"):
+        runtime.drop_device_resource(r)
+    # the Filter -> Project leg, alternating with a built checkout of the parent when OPS_PARENT names one
+    parent = os.environ.get("OPS_PARENT")
+    for k in range(3):
+        print(f"== Filter -> Project, this tree, pass {k + 1}: expr_vm {filter_project_leg().get('expr_vm', 0) / 1000:.3f} ms")
+        if parent:
+            out = subprocess.run([sys.executable, os.path.join(parent, "tools", "bench_ops.py"), "filter_project"], capture_output=True, text=True,
+                                 cwd=parent, env=dict(os.environ, OPS_ROWS=str(N))).stdout
+            ms = re.search(r"expr_vm\s+([0-9.]+) ms", out)
+            print(f"== Filter -> Project, parent tree, pass {k + 1}: expr_vm {ms.group(1) if ms else '?'} ms")
+
 
 if "scalar" in which:
     import subprocess
