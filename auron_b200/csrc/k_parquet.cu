@@ -23,37 +23,68 @@ namespace auron {
         launch_count(ctx);           \
     } while (0)
 
-__device__ __forceinline__ void store_converted(const PqColumnArgs& a, const uint8_t* src, int64_t row) {
-    // src points at one physical value (little-endian INT32/INT64/FLOAT/DOUBLE, big-endian FLBA)
+// FIXED_LEN_BYTE_ARRAY decimal: n big-endian two's complement bytes -> decimal128 (hi:lo)
+__device__ __forceinline__ void load_flba(const uint8_t* src, int n, uint64_t& lo, uint64_t& hi) {
+    hi = (src[0] & 0x80) ? ~0ull : 0ull;
+    lo = hi;
+    for (int i = 0; i < n; i++) {
+        hi = (hi << 8) | (lo >> 56);
+        lo = (lo << 8) | src[i];
+    }
+}
+__device__ __forceinline__ void store_i128(const PqColumnArgs& a, int64_t row, uint64_t lo, uint64_t hi) {
+    ((uint64_t*)a.out)[2 * row] = lo;
+    ((uint64_t*)a.out)[2 * row + 1] = hi;
+}
+// The conversions that scale (PQ_CV_TS_MUL, PQ_CV_TS_DIV, PQ_CV_DEC).
+// False when the product leaves int64 (a zero is stored and the row must be NULL).
+__device__ __forceinline__ bool store_scaled(const PqColumnArgs& a, const uint8_t* src, int64_t row) {
+    if (a.conv != PQ_CV_DEC) {   // INT64 timestamps
+        const int64_t x = (int64_t)ld_u64_unaligned(src), m = (int64_t)a.conv_mul;
+        if (a.conv == PQ_CV_TS_DIV) {
+            ((int64_t*)a.out)[row] = x / m;   // truncating, as arrow divides
+            return true;
+        }
+        const bool ok = x <= INT64_MAX / m && x >= INT64_MIN / m;   // arrow's safe cast: NULL where the product leaves int64
+        ((int64_t*)a.out)[row] = ok ? x * m : 0;
+        return ok;
+    }
+    // decimal on INT32 / INT64 / FLBA x 10^k; the host admits only targets wide enough for the product
+    uint64_t lo, hi;
+    if (a.phys_type == 7) load_flba(src, a.type_length, lo, hi);
+    else {
+        const int64_t x = a.phys_type == 1 ? (int64_t)(int32_t)ld_u32_unaligned(src) : (int64_t)ld_u64_unaligned(src);
+        lo = (uint64_t)x;
+        hi = x < 0 ? ~0ull : 0ull;
+    }
+    const unsigned __int128 r = (((unsigned __int128)hi << 64) | lo) * (((unsigned __int128)a.conv_mul_hi << 64) | a.conv_mul);   // two's complement: the low 128 bits
+    store_i128(a, row, (uint64_t)r, (uint64_t)(r >> 64));
+    return true;
+}
+// Converts the physical value at src (little-endian INT32/INT64/FLOAT/DOUBLE, big-endian FLBA) as a.conv says and stores it at `row`.
+// False when the value has no representation in the table's type (PQ_CV_TS_MUL overflow): a zero is stored and the row must be NULL.
+__device__ __forceinline__ bool store_converted(const PqColumnArgs& a, const uint8_t* src, int64_t row) {
+    if (a.conv >= PQ_CV_TS_MUL) return store_scaled(a, src, row);
     switch (a.phys_type) {
         case 1: case 4: {   // INT32 / FLOAT
-            uint32_t v = ld_u32_unaligned(src);
-            switch (a.out_type) {
-                case T_INT8: ((int8_t*)a.out)[row] = (int8_t)v; break;
-                case T_INT16: ((int16_t*)a.out)[row] = (int16_t)v; break;
-                case T_INT32: case T_DATE32: case T_FLOAT32: ((uint32_t*)a.out)[row] = v; break;
-                case T_INT64: case T_TIMESTAMP: case T_DATE64: ((int64_t*)a.out)[row] = (int64_t)(int32_t)v; break;
-                case T_FLOAT64: ((double*)a.out)[row] = (double)__int_as_float((int)v); break;
-                case T_DECIMAL128: {   // scan/mod.rs:131-136: value copy, no rescale
-                    int64_t s = (int64_t)(int32_t)v;
-                    ((int64_t*)a.out)[2 * row] = s;
-                    ((int64_t*)a.out)[2 * row + 1] = s < 0 ? -1 : 0;
-                    break;
-                }
+            const uint32_t v = ld_u32_unaligned(src);
+            const int64_t x = a.conv == PQ_CV_ZEXT ? (int64_t)v : (int64_t)(int32_t)v;
+            if (a.conv == PQ_CV_I32_F64) ((double*)a.out)[row] = (double)(int32_t)v;
+            else if (a.conv == PQ_CV_F32_F64) ((double*)a.out)[row] = (double)__int_as_float((int)v);
+            else switch (a.out_width) {   // PQ_CV_COPY (narrowing stores only where the annotation says the value fits), SEXT, ZEXT
+                case 1: ((int8_t*)a.out)[row] = (int8_t)x; break;
+                case 2: ((int16_t*)a.out)[row] = (int16_t)x; break;
+                case 4: ((uint32_t*)a.out)[row] = v; break;
+                case 8: ((int64_t*)a.out)[row] = x; break;
+                case 16: store_i128(a, row, (uint64_t)x, x < 0 ? ~0ull : 0ull); break;   // scan/mod.rs:131-136: value copy, no rescale
             }
-            break;
+            return true;
         }
         case 2: case 5: {   // INT64 / DOUBLE
-            uint64_t v = ld_u64_unaligned(src);
-            switch (a.out_type) {
-                case T_INT32: case T_DATE32: ((int32_t*)a.out)[row] = (int32_t)v; break;
-                case T_DECIMAL128:
-                    ((uint64_t*)a.out)[2 * row] = v;
-                    ((int64_t*)a.out)[2 * row + 1] = ((int64_t)v) < 0 ? -1 : 0;
-                    break;
-                default: ((uint64_t*)a.out)[row] = v; break;
-            }
-            break;
+            const uint64_t v = ld_u64_unaligned(src);
+            if (a.out_width == 16) store_i128(a, row, v, (int64_t)v < 0 ? ~0ull : 0ull);
+            else ((uint64_t*)a.out)[row] = v;
+            return true;
         }
         case 3: {   // INT96 timestamp: 8 bytes nanoseconds of the day (LE) + 4 bytes Julian day (LE) -> the output column's unit
             const int64_t nanos = (int64_t)ld_u64_unaligned(src);
@@ -66,23 +97,16 @@ __device__ __forceinline__ void store_converted(const PqColumnArgs& a, const uin
                 default: v = days * 86400000000ll + nanos / 1000ll; break;
             }
             ((int64_t*)a.out)[row] = v;
-            break;
+            return true;
         }
-        case 7: {   // FIXED_LEN_BYTE_ARRAY decimal: big-endian two's complement
-            int n = a.type_length;
-            uint64_t hi = (src[0] & 0x80) ? ~0ull : 0ull, lo = hi;
-            for (int i = 0; i < n; i++) {
-                hi = (hi << 8) | (lo >> 56);
-                lo = (lo << 8) | src[i];
-            }
-            if (a.out_type == T_DECIMAL128) {
-                ((uint64_t*)a.out)[2 * row] = lo;
-                ((uint64_t*)a.out)[2 * row + 1] = hi;
-            } else if (a.out_type == T_INT64) ((uint64_t*)a.out)[row] = lo;
-            else ((uint32_t*)a.out)[row] = (uint32_t)lo;
-            break;
+        case 7: {   // FIXED_LEN_BYTE_ARRAY decimal at its own scale (the host admits decimal128 targets only)
+            uint64_t lo, hi;
+            load_flba(src, a.type_length, lo, hi);
+            store_i128(a, row, lo, hi);
+            return true;
         }
     }
+    return true;
 }
 __device__ __forceinline__ void store_zero(const PqColumnArgs& a, int64_t row) {
     switch (a.out_width) {
@@ -403,9 +427,10 @@ __global__ void __launch_bounds__(PQ_WARPS * 32) pq_decode_tiles_fast_kernel(PqL
     s_pref[wid][lane] = prefix;
     __syncwarp();
     // specialised inner loops for the common fixed-width cases: no per-row type switches, rank base from shared memory
-    const bool same4 = a.mode == PQ_MODE_VALUES && width == 4 && a.out_width == 4 && (a.phys_type == 1 || a.phys_type == 4);
-    const bool same8 = a.mode == PQ_MODE_VALUES && width == 8 && a.out_width == 8 && (a.phys_type == 2 || a.phys_type == 5);
-    const bool widen = a.mode == PQ_MODE_VALUES && a.phys_type == 1 && (a.out_type == T_INT64 || a.out_type == T_TIMESTAMP || a.out_type == T_DATE64);
+    // (copies and sign extensions only: every other conversion goes through store_converted)
+    const bool same4 = a.mode == PQ_MODE_VALUES && a.conv == PQ_CV_COPY && width == 4 && a.out_width == 4 && (a.phys_type == 1 || a.phys_type == 4);
+    const bool same8 = a.mode == PQ_MODE_VALUES && a.conv == PQ_CV_COPY && width == 8 && a.out_width == 8 && (a.phys_type == 2 || a.phys_type == 5);
+    const bool widen = a.mode == PQ_MODE_VALUES && a.conv == PQ_CV_SEXT && a.phys_type == 1 && a.out_width == 8;
     if (same4 || widen) {
         // value r (dictionary index, or PLAIN ordinal within the tile) is the 32-bit word at base + 4r; the base is
         // not 4-byte aligned in general (page payloads sit at arbitrary file offsets): one uniform funnel shift
@@ -479,30 +504,37 @@ __global__ void __launch_bounds__(PQ_WARPS * 32) pq_decode_tiles_fast_kernel(PqL
                 if (32 * (j0 + u) + (int)lane < n) ((uint64_t*)a.out)[out0 + 32 * (j0 + u) + lane] = v[u];
         }
     } else
-    for (int j = 0; j * 32 < n; j++) {
-        int i = 32 * j + (int)lane;
-        bool active = i < n;
-        uint32_t wj = s_w[wid][j];
-        int pj = __shfl_sync(FULL_MASK, prefix, j);
-        bool valid = active && ((wj >> lane) & 1u);
-        int rank = pj + __popc(wj & lanemask_lt());
-        int64_t row = out0 + i;
-        if (!active) continue;
-        if (a.mode == PQ_MODE_INDEX) {
-            uint32_t di = dict ? s_vals[wid][rank] : 0;
-            if (di >= (uint32_t)dd.num_values) di = 0;
-            a.out_idx[row] = valid ? (dict ? dd.value_base + (int32_t)di : pg.plain_value_base + (int32_t)(tl.v0 + rank)) : -1;
-        } else if (valid) {
-            const uint8_t* src;
-            if (dict) {
-                uint32_t di = s_vals[wid][rank];
-                if (di >= (uint32_t)dd.num_values) di = 0;   // corrupt index guard
-                src = dd.data + (int64_t)di * width;
-            } else src = vals + (tl.v0 + rank) * width;
-            store_converted(a, src, row);
-        } else {
-            store_zero(a, row);
+    {
+        for (int j = 0; j * 32 < n; j++) {
+            int i = 32 * j + (int)lane;
+            bool active = i < n;
+            uint32_t wj = s_w[wid][j];
+            int pj = __shfl_sync(FULL_MASK, prefix, j);
+            bool valid = active && ((wj >> lane) & 1u);
+            int rank = pj + __popc(wj & lanemask_lt());
+            int64_t row = out0 + i;
+            bool ok = true;
+            if (active && a.mode == PQ_MODE_INDEX) {
+                uint32_t di = dict ? s_vals[wid][rank] : 0;
+                if (di >= (uint32_t)dd.num_values) di = 0;
+                a.out_idx[row] = valid ? (dict ? dd.value_base + (int32_t)di : pg.plain_value_base + (int32_t)(tl.v0 + rank)) : -1;
+            } else if (valid) {
+                const uint8_t* src;
+                if (dict) {
+                    uint32_t di = s_vals[wid][rank];
+                    if (di >= (uint32_t)dd.num_values) di = 0;   // corrupt index guard
+                    src = dd.data + (int64_t)di * width;
+                } else src = vals + (tl.v0 + rank) * width;
+                ok = store_converted(a, src, row);
+            } else if (active) {
+                store_zero(a, row);
+            }
+            if (a.conv == PQ_CV_TS_MUL) {   // values the conversion cannot represent become NULL (the column has a validity buffer)
+                const uint32_t bad = __ballot_sync(FULL_MASK, !ok);
+                if (lane == 0 && bad) s_w[wid][j] = wj & ~bad;
+            }
         }
+        __syncwarp();
     }
     // ---- 4. validity words of the output (tile rows are not 32-aligned in general)
     if (a.out_valid) {

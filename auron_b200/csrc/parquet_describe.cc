@@ -59,7 +59,9 @@ std::string describe(const char* path) {
     for (size_t i = 0; i < md.schema.size(); i++) {
         const auto& e = md.schema[i];
         o << (i ? "," : "") << "{\"name\":" << quote(e.name) << ",\"type\":" << e.type << ",\"type_length\":" << e.type_length << ",\"repetition\":" << e.repetition
-          << ",\"num_children\":" << e.num_children << ",\"converted_type\":" << e.converted_type << ",\"scale\":" << e.scale << ",\"precision\":" << e.precision << "}";
+          << ",\"num_children\":" << e.num_children << ",\"converted_type\":" << e.converted_type << ",\"scale\":" << e.scale << ",\"precision\":" << e.precision
+          << ",\"has_logical_type\":" << (e.has_logical_type ? "true" : "false") << ",\"logical\":" << e.logical << ",\"ts_unit\":" << e.ts_unit
+          << ",\"ts_utc\":" << (e.ts_utc ? "true" : "false") << ",\"int_bits\":" << e.int_bits << ",\"int_signed\":" << (e.int_signed ? "true" : "false") << "}";
     }
     o << "],\"row_groups\":[";
     for (size_t g = 0; g < md.row_groups.size(); g++) {

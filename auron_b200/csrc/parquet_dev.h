@@ -24,6 +24,19 @@ struct PqDict {
     int32_t value_base;       // strings: position of entry 0 in the value table
 };
 enum { PQ_MODE_VALUES = 0, PQ_MODE_INDEX = 1 };
+// How one physical value becomes one value of the table's type, decided once per column on the host (scan_parquet.cc,
+// conversion_of: the table of DESIGN section 4, "Parquet column conversions")
+enum PqConv {
+    PQ_CV_COPY = 0,     // the value as it is, stored at the output's width (also INT96 -> timestamp, booleans, byte arrays)
+    PQ_CV_SEXT = 1,     // a signed INT32 / INT64 sign-extended to a wider integer, or to decimal128 as a value copy
+                        //   (scan/mod.rs:131-136; also a decimal read at its own scale)
+    PQ_CV_ZEXT = 2,     // an unsigned INT32 (UINT 8 / 16 / 32) zero-extended to a wider signed integer
+    PQ_CV_I32_F64 = 3,  // a signed INT32 as the float64 of the same value
+    PQ_CV_F32_F64 = 4,  // FLOAT widened to float64
+    PQ_CV_TS_MUL = 5,   // INT64 timestamp x conv_mul into a finer unit; NULL when the product leaves int64
+    PQ_CV_TS_DIV = 6,   // INT64 timestamp / conv_mul into a coarser unit, truncating toward zero
+    PQ_CV_DEC = 7,      // a decimal on INT32 / INT64 / FLBA x (conv_mul_hi:conv_mul) > 1 into decimal128 (exact: the target is wide enough)
+};
 struct PqColumnArgs {
     const PqPage* pages;
     const PqDict* dicts;
@@ -32,7 +45,9 @@ struct PqColumnArgs {
     int32_t out_type, out_width;
     int32_t max_def;
     int32_t mode;
-    int32_t out_unit, pad0;   // T_TIMESTAMP output: 0 s, 1 ms, 2 us, 3 ns (INT96 pages are converted to it)
+    int32_t out_unit;   // T_TIMESTAMP output: 0 s, 1 ms, 2 us, 3 ns (INT96 pages are converted to it)
+    int32_t conv;       // PqConv
+    uint64_t conv_mul, conv_mul_hi;
     void* out;
     uint32_t* out_valid;
     int32_t* out_idx;

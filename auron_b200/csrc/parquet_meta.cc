@@ -106,6 +106,79 @@ struct TReader {
     }
 };
 
+// union LogicalType (parquet.thrift): 1 STRING, 5 DECIMAL{1 scale, 2 precision}, 6 DATE, 8 TIMESTAMP{1 isAdjustedToUTC, 2 unit},
+// 10 INTEGER{1 bitWidth (i8), 2 isSigned}; TimeUnit: 1 MILLIS, 2 MICROS, 3 NANOS.  Every other member is LK_OTHER.
+void read_logical_type(TReader& r, SchemaElement& e) {
+    int16_t id, last = 0;
+    int t;
+    e.has_logical_type = true;
+    e.logical = LK_OTHER;
+    while (r.field(&id, &t, &last)) {
+        if (t != 12) {
+            r.skip(t);
+            continue;
+        }
+        int16_t i2, l2 = 0;
+        int t2;
+        switch (id) {
+            case 1: e.logical = LK_STRING; r.skip(t); break;
+            case 6: e.logical = LK_DATE; r.skip(t); break;
+            case 5:
+                e.logical = LK_DECIMAL;
+                while (r.field(&i2, &t2, &l2)) {
+                    if (i2 == 1 && t2 == 5) e.scale = (int32_t)r.zigzag();
+                    else if (i2 == 2 && t2 == 5) e.precision = (int32_t)r.zigzag();
+                    else r.skip(t2);
+                }
+                break;
+            case 8:
+                e.logical = LK_TIMESTAMP;
+                while (r.field(&i2, &t2, &l2)) {
+                    if (i2 == 1 && (t2 == 1 || t2 == 2)) e.ts_utc = t2 == 1;   // a bool's value is its field type
+                    else if (i2 == 2 && t2 == 12) {
+                        int16_t i3, l3 = 0;
+                        int t3;
+                        while (r.field(&i3, &t3, &l3)) {
+                            if (i3 >= 1 && i3 <= 3) e.ts_unit = i3;
+                            r.skip(t3);
+                        }
+                    } else r.skip(t2);
+                }
+                if (e.ts_unit < 0) e.logical = LK_OTHER;
+                break;
+            case 10:
+                e.logical = LK_INTEGER;
+                while (r.field(&i2, &t2, &l2)) {
+                    if (i2 == 1 && t2 == 3) e.int_bits = (int8_t)r.byte();
+                    else if (i2 == 2 && (t2 == 1 || t2 == 2)) e.int_signed = t2 == 1;
+                    else r.skip(t2);
+                }
+                if (e.int_bits != 8 && e.int_bits != 16 && e.int_bits != 32 && e.int_bits != 64) e.logical = LK_OTHER;
+                break;
+            default: r.skip(t);
+        }
+    }
+}
+// ConvertedType (parquet.thrift) -> annotation, for files without a LogicalType
+void logical_from_converted(SchemaElement& e) {
+    const int c = e.converted_type;
+    if (c < 0) return;
+    if (c == 0) e.logical = LK_STRING;
+    else if (c == 5) e.logical = LK_DECIMAL;
+    else if (c == 6) e.logical = LK_DATE;
+    else if (c == 9 || c == 10) {   // TIMESTAMP_MILLIS / TIMESTAMP_MICROS: adjusted to UTC (LogicalTypes.md, "Backward compatibility")
+        e.logical = LK_TIMESTAMP;
+        e.ts_unit = c == 9 ? 1 : 2;
+        e.ts_utc = true;
+    } else if (c >= 11 && c <= 18) {   // UINT_8 .. UINT_64, INT_8 .. INT_64
+        e.logical = LK_INTEGER;
+        e.int_signed = c >= 15;
+        e.int_bits = 8 << ((c - 11) % 4);
+    } else if (c >= 1 && c <= 4) {
+        e.logical = c == 4 ? LK_STRING : LK_OTHER;   // ENUM is a string; MAP / LIST belong to groups
+    } else e.logical = LK_OTHER;
+}
+
 SchemaElement read_schema_element(TReader& r) {
     SchemaElement e;
     int16_t id, last = 0;
@@ -120,9 +193,14 @@ SchemaElement read_schema_element(TReader& r) {
             case 6: e.converted_type = (int32_t)r.zigzag(); break;
             case 7: e.scale = (int32_t)r.zigzag(); break;
             case 8: e.precision = (int32_t)r.zigzag(); break;
+            case 10:
+                if (t == 12) read_logical_type(r, e);
+                else r.skip(t);
+                break;
             default: r.skip(t);
         }
     }
+    if (!e.has_logical_type) logical_from_converted(e);
     return e;
 }
 Statistics read_statistics(TReader& r) {
@@ -141,8 +219,8 @@ Statistics read_statistics(TReader& r) {
             default: r.skip(t);
         }
     }
-    if (!s.has_max && has_old_max) { s.max_value = old_max; s.has_max = true; }
-    if (!s.has_min && has_old_min) { s.min_value = old_min; s.has_min = true; }
+    if (!s.has_max && has_old_max) { s.max_value = old_max; s.has_max = s.legacy_max = true; }
+    if (!s.has_min && has_old_min) { s.min_value = old_min; s.has_min = s.legacy_min = true; }
     return s;
 }
 ColumnMeta read_column_meta(TReader& r) {
@@ -231,6 +309,18 @@ FileMeta parse_file_meta(const uint8_t* buf, size_t len) {
             default: r.skip(t);
         }
     }
+    // The legacy min / max fields were written in signed byte order whatever the column's type: a reader must ignore them unless
+    // the column's sort order is signed (parquet.thrift, Statistics).  Column chunk c belongs to the c-th leaf of the schema.
+    std::vector<const SchemaElement*> leaves;
+    for (size_t i = 1; i < m.schema.size(); i++)
+        if (m.schema[i].num_children == 0) leaves.push_back(&m.schema[i]);
+    for (auto& rg : m.row_groups)
+        for (size_t c = 0; c < rg.columns.size(); c++) {
+            Statistics& s = rg.columns[c].stats;
+            if (c < leaves.size() && leaves[c]->signed_order()) continue;
+            if (s.legacy_min) s.has_min = s.legacy_min = false, s.min_value.clear();
+            if (s.legacy_max) s.has_max = s.legacy_max = false, s.max_value.clear();
+        }
     return m;
 }
 

@@ -17,12 +17,27 @@ enum Encoding { ENC_PLAIN = 0, ENC_PLAIN_DICTIONARY = 2, ENC_RLE = 3, ENC_BIT_PA
 enum Codec { CODEC_UNCOMPRESSED = 0, CODEC_SNAPPY = 1, CODEC_GZIP = 2, CODEC_LZ4 = 5, CODEC_ZSTD = 6, CODEC_LZ4_RAW = 7 };
 enum PageType { PAGE_DATA = 0, PAGE_INDEX = 1, PAGE_DICTIONARY = 2, PAGE_DATA_V2 = 3 };
 
+// The annotation of a column: SchemaElement.logicalType (field 10) when present, else the one its converted_type (field 6) implies
+enum LogicalKind { LK_NONE = 0, LK_STRING = 1, LK_DECIMAL = 2, LK_DATE = 3, LK_TIMESTAMP = 4, LK_INTEGER = 5, LK_OTHER = 6 };
 struct SchemaElement {
     int32_t type = -1, type_length = 0, repetition = 0, num_children = 0, converted_type = -1, scale = 0, precision = 0;
     std::string name;
+    bool has_logical_type = false;   // field 10 was present
+    int32_t logical = LK_NONE;
+    int32_t ts_unit = -1;            // LK_TIMESTAMP: 1 ms, 2 us, 3 ns (the coding of DType::unit)
+    bool ts_utc = false;             // LK_TIMESTAMP: isAdjustedToUTC
+    int32_t int_bits = 0;            // LK_INTEGER: 8, 16, 32 or 64
+    bool int_signed = true;          // LK_INTEGER
+    // min / max statistics are ordered as signed values (the only order the legacy min / max fields may be read in)
+    bool signed_order() const {
+        if (logical == LK_INTEGER) return int_signed;
+        if (logical == LK_DECIMAL) return true;
+        return logical != LK_STRING && logical != LK_OTHER && type != 3 && type != 6 && type != 7 && type >= 0;
+    }
 };
 struct Statistics {
     bool has_min = false, has_max = false, has_null_count = false;
+    bool legacy_min = false, legacy_max = false;   // taken from the deprecated min / max fields (1, 2)
     std::string min_value, max_value;
     int64_t null_count = 0;
 };

@@ -286,6 +286,10 @@ struct ParquetScanExec : Operator, FusedScanSource {
         rg_pos = 0;
         cur = fs;
     }
+    struct Conv {   // a PqConv with its factor (conversion_of)
+        int32_t kind = PQ_CV_COPY;
+        uint64_t mul = 1, mul_hi = 0;
+    };
     // can no row of this row group satisfy the pruning intervals?  (min / max statistics of INT32 / INT64 chunks; a chunk whose
     // values are all NULL satisfies no comparison)
     bool row_group_pruned(const FileState& f, const pq::RowGroup& rg) const {
@@ -297,19 +301,11 @@ struct ParquetScanExec : Operator, FusedScanSource {
             const pq::ColumnMeta& cm = rg.columns[(size_t)leaf_index];
             const pq::Statistics& st = cm.stats;
             if (st.has_null_count && st.null_count == cm.num_values && cm.num_values > 0) return true;
-            const int pt = f.leaves[(size_t)li].el.type;
-            const size_t w = pt == pq::PT_INT32 ? 4 : pt == pq::PT_INT64 ? 8 : 0;
-            if (!w || !st.has_min || !st.has_max || st.min_value.size() != w || st.max_value.size() != w) continue;
-            int64_t mn, mx;
-            if (w == 4) {
-                int32_t a, b;
-                memcpy(&a, st.min_value.data(), 4);
-                memcpy(&b, st.max_value.data(), 4);
-                mn = a, mx = b;
-            } else {
-                memcpy(&mn, st.min_value.data(), 8);
-                memcpy(&mx, st.max_value.data(), 8);
-            }
+            const pq::SchemaElement& el = f.leaves[(size_t)li].el;
+            Conv cv;   // (a column the table cannot read fails when it is projected, not here)
+            if (!try_conversion(el, table_schema.fields[(size_t)prune_cols[i]].type, &cv)) continue;
+            int64_t mn, mx;   // bounds in the table's type: the pruning intervals are
+            if (!converted_bounds(el, cv, st, &mn, &mx)) continue;
             if (mx < prune_lo[i] || mn > prune_hi[i]) return true;
         }
         return false;
@@ -336,8 +332,12 @@ struct ParquetScanExec : Operator, FusedScanSource {
             }
             int li = find_leaf(f, table_schema.fields[pj].name);
             if (li < 0) s += "-;";
-            else s += std::to_string(f.leaves[li].leaf_index) + ":" + std::to_string(f.leaves[li].el.type) + ":" + std::to_string(f.leaves[li].el.repetition) +
-                      ":" + std::to_string(f.leaves[li].el.type_length) + ";";
+            else {
+                const pq::SchemaElement& el = f.leaves[li].el;   // (the annotation decides the conversion)
+                s += std::to_string(f.leaves[li].leaf_index) + ":" + std::to_string(el.type) + ":" + std::to_string(el.repetition) + ":" + std::to_string(el.type_length) +
+                     ":" + std::to_string(el.logical) + ":" + std::to_string(el.ts_unit) + ":" + std::to_string(el.int_bits) + ":" + std::to_string(el.int_signed) + ":" +
+                     std::to_string(el.precision) + ":" + std::to_string(el.scale) + ";";
+            }
         }
         return s;
     }
@@ -384,6 +384,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
         int part_col = -1;   // >= 0: column of the partition schema (no file column at all)
         pq::SchemaElement el;
         bool is_string = false;
+        Conv cv;   // physical value -> table type
         std::vector<PqPage> pages;
         std::vector<PqDict> dicts;
         std::vector<PqByteSection> secs;
@@ -581,7 +582,8 @@ struct ParquetScanExec : Operator, FusedScanSource {
             const bool delta_ints = h.encoding == pq::ENC_DELTA_BINARY_PACKED && (el.type == pq::PT_INT32 || el.type == pq::PT_INT64);
             AURON_CHECK(h.encoding == pq::ENC_PLAIN || ((h.encoding == pq::ENC_RLE_DICTIONARY || h.encoding == pq::ENC_PLAIN_DICTIONARY) && cur_dict >= 0) ||
                             (h.encoding == pq::ENC_RLE && el.type == pq::PT_BOOLEAN) || delta_ints || delta_strings,
-                        "parquet encoding " + std::to_string(h.encoding) + " is not supported (PLAIN, RLE_DICTIONARY, RLE booleans and the DELTA encodings are)");
+                        "parquet encoding " + std::to_string(h.encoding) + (h.encoding == 9 ? " (BYTE_STREAM_SPLIT)" : "") + " of column " + el.name +
+                            " is not supported (PLAIN, RLE_DICTIONARY, RLE booleans and the DELTA encodings are)");
             if (delta_ints) {   // transcribed on the device, after the sections of the page are known (pq_delta_to_plain)
                 pg.encoding = pq::ENC_PLAIN;
                 pg.delta_dst16 = (int32_t)(out.gpu_unc_bytes / 16) + 1;
@@ -665,20 +667,113 @@ struct ParquetScanExec : Operator, FusedScanSource {
             default: return 0;
         }
     }
-    static void check_types(const pq::SchemaElement& el, const DType& t) {
+    // ---- one conversion per column: (physical type, annotation, table type) -> PqConv.  The reference reads the file's Arrow type
+    // and AuronSchemaAdapter (scan/mod.rs:103-160) casts it to the table's; the pairs below are those whose cast is exact, plus the
+    // integer -> decimal value copy of scan/mod.rs:131-136.  Everything else fails (DESIGN section 4, "Parquet column conversions").
+    // false for a pair outside the table
+    static bool try_conversion(const pq::SchemaElement& el, const DType& t, Conv* out) {
+        Conv cv;
         bool ok = false;
-        switch (el.type) {
-            case pq::PT_BOOLEAN: ok = t.id == T_BOOL; break;
-            case pq::PT_INT32: ok = t.id == T_INT8 || t.id == T_INT16 || t.id == T_INT32 || t.id == T_DATE32 || t.id == T_INT64 || t.id == T_DECIMAL128 || t.id == T_FLOAT64; break;
-            case pq::PT_INT64: ok = t.id == T_INT64 || t.id == T_TIMESTAMP || t.id == T_DATE64 || t.id == T_DECIMAL128 || t.id == T_INT32; break;
-            case pq::PT_INT96: ok = t.id == T_TIMESTAMP; break;   // Spark's legacy timestamp encoding (parquet_exec.rs:192 coerces it)
-            case pq::PT_FLOAT: ok = t.id == T_FLOAT32 || t.id == T_FLOAT64; break;
-            case pq::PT_DOUBLE: ok = t.id == T_FLOAT64; break;
-            case pq::PT_BYTE_ARRAY: ok = t.is_varlen(); break;
-            case pq::PT_FLBA: ok = t.id == T_DECIMAL128 && el.type_length <= 16; break;
-            default: ok = false;
+        auto kind = [&](int32_t k) {
+            cv.kind = k;
+            ok = true;
+        };
+        const int lk = el.logical;
+        const bool is_int_target = t.id == T_INT8 || t.id == T_INT16 || t.id == T_INT32 || t.id == T_INT64;
+        if (lk == pq::LK_DECIMAL) {
+            // decimal(p1, s1) -> decimal(p2, s2): x 10^(s2 - s1) when no digit is lost and the integer part fits (always exact)
+            const bool storage = (el.type == pq::PT_INT32 && el.precision <= 9) || (el.type == pq::PT_INT64 && el.precision <= 18) ||
+                                 (el.type == pq::PT_FLBA && el.type_length >= 1 && el.type_length <= 16);
+            if (storage && t.id == T_DECIMAL128 && el.precision >= 1 && el.scale >= 0 && t.scale >= el.scale && t.precision - t.scale >= el.precision - el.scale) {
+                unsigned __int128 m = 1;
+                for (int i = el.scale; i < t.scale; i++) m *= 10;
+                kind(m == 1 ? PQ_CV_SEXT : PQ_CV_DEC);   // (at its own scale: the value copy)
+                cv.mul = (uint64_t)m;
+                cv.mul_hi = (uint64_t)(m >> 64);
+            }
+        } else {
+            switch (el.type) {
+                case pq::PT_BOOLEAN: if (t.id == T_BOOL && lk == pq::LK_NONE) kind(PQ_CV_COPY); break;
+                case pq::PT_INT32: {
+                    const bool sgn = lk == pq::LK_NONE || (lk == pq::LK_INTEGER && el.int_signed && el.int_bits <= 32);
+                    const int bits = lk == pq::LK_INTEGER ? el.int_bits : 32;
+                    if (lk == pq::LK_INTEGER && !el.int_signed && el.int_bits <= 32) {
+                        if (is_int_target && 8 * t.width() > bits) kind(PQ_CV_ZEXT);   // UINT_n into a strictly wider signed integer
+                    } else if (sgn || lk == pq::LK_DATE) {
+                        if ((t.id == T_INT8 || t.id == T_INT16) && sgn && bits <= 8 * t.width()) kind(PQ_CV_COPY);
+                        else if (t.id == T_INT32 || t.id == T_DATE32) kind(PQ_CV_COPY);
+                        else if (t.id == T_INT64) kind(PQ_CV_SEXT);
+                        else if (t.id == T_FLOAT64 && sgn) kind(PQ_CV_I32_F64);
+                        else if (t.id == T_DECIMAL128 && sgn) kind(PQ_CV_SEXT);
+                    }
+                    break;
+                }
+                case pq::PT_INT64:
+                    if (lk == pq::LK_TIMESTAMP) {
+                        if (t.id == T_INT64) kind(PQ_CV_COPY);   // the stored count, as arrow casts a timestamp to int64
+                        else if (t.id == T_TIMESTAMP && t.unit >= 0 && t.unit <= 3) {
+                            const int d = t.unit - el.ts_unit;
+                            uint64_t m = 1;
+                            for (int i = 0; i < 3 * (d < 0 ? -d : d); i++) m *= 10;
+                            kind(d == 0 ? PQ_CV_COPY : d > 0 ? PQ_CV_TS_MUL : PQ_CV_TS_DIV);
+                            cv.mul = m;
+                        }
+                    } else if (lk == pq::LK_NONE || (lk == pq::LK_INTEGER && el.int_signed)) {
+                        if (t.id == T_INT64 || t.id == T_DATE64 || t.id == T_TIMESTAMP) kind(PQ_CV_COPY);   // (a plain int64 is a count in the table's unit)
+                        else if (t.id == T_DECIMAL128) kind(PQ_CV_SEXT);
+                    }
+                    break;
+                case pq::PT_INT96: if (t.id == T_TIMESTAMP) kind(PQ_CV_COPY); break;   // Spark's legacy timestamp encoding (parquet_exec.rs:192 coerces it)
+                case pq::PT_FLOAT: if (t.id == T_FLOAT32) kind(PQ_CV_COPY); else if (t.id == T_FLOAT64) kind(PQ_CV_F32_F64); break;
+                case pq::PT_DOUBLE: if (t.id == T_FLOAT64) kind(PQ_CV_COPY); break;
+                case pq::PT_BYTE_ARRAY: if (t.is_varlen()) kind(PQ_CV_COPY); break;
+                default: break;
+            }
         }
-        AURON_CHECK(ok, "cannot read parquet column " + el.name + " (physical type " + std::to_string(el.type) + ") as " + t.str());
+        *out = cv;
+        return ok;
+    }
+    static Conv conversion_of(const pq::SchemaElement& el, const DType& t) {
+        Conv cv;
+        if (try_conversion(el, t, &cv)) return cv;
+        const int lk = el.logical;
+        static const char* kLogical[] = {"", ", STRING", ", DECIMAL", ", DATE", ", TIMESTAMP", ", INTEGER", ", other annotation"};
+        std::string ann = kLogical[lk >= 0 && lk <= 6 ? lk : 6];
+        if (lk == pq::LK_DECIMAL) ann += "(" + std::to_string(el.precision) + "," + std::to_string(el.scale) + ")";
+        if (lk == pq::LK_INTEGER) ann += std::string("(") + std::to_string(el.int_bits) + (el.int_signed ? ",signed)" : ",unsigned)");
+        if (lk == pq::LK_TIMESTAMP) ann += el.ts_unit == 1 ? "(ms)" : el.ts_unit == 2 ? "(us)" : "(ns)";
+        fail("cannot read parquet column " + el.name + " (physical type " + std::to_string(el.type) + ann + ") as " + t.str());
+    }
+    // Column-chunk min / max in the table's type (Statistics.min_value / max_value are PLAIN-encoded: little-endian two's complement).
+    // False when they do not bound the converted values (no statistics, or a conversion that is not monotone into an integer).
+    static bool converted_bounds(const pq::SchemaElement& el, const Conv& cv, const pq::Statistics& st, int64_t* mn, int64_t* mx) {
+        const size_t w = el.type == pq::PT_INT32 ? 4 : el.type == pq::PT_INT64 ? 8 : 0;
+        if (!w || !st.has_min || !st.has_max || st.min_value.size() != w || st.max_value.size() != w) return false;
+        auto read = [&](const std::string& s) -> int64_t {
+            if (w == 8) {
+                int64_t v;
+                memcpy(&v, s.data(), 8);
+                return v;
+            }
+            uint32_t v;
+            memcpy(&v, s.data(), 4);
+            return cv.kind == PQ_CV_ZEXT ? (int64_t)v : (int64_t)(int32_t)v;   // an unsigned column's statistics are unsigned
+        };
+        int64_t a = read(st.min_value), b = read(st.max_value);
+        switch (cv.kind) {
+            case PQ_CV_COPY: case PQ_CV_SEXT: case PQ_CV_ZEXT: break;
+            case PQ_CV_TS_MUL: {   // a bound whose product leaves int64 is dropped: those values are NULL after the conversion
+                const int64_t m = (int64_t)cv.mul;
+                a = a < INT64_MIN / m ? INT64_MIN : a > INT64_MAX / m ? INT64_MAX : a * m;
+                b = b > INT64_MAX / m ? INT64_MAX : b < INT64_MIN / m ? INT64_MIN : b * m;
+                break;
+            }
+            case PQ_CV_TS_DIV: a /= (int64_t)cv.mul, b /= (int64_t)cv.mul; break;   // truncation is monotone
+            default: return false;
+        }
+        *mn = a;
+        *mx = b;
+        return true;
     }
 
     const PqDecompResult* decomp_results = nullptr;   // results of the current batch's decompression launch (device)
@@ -818,7 +913,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
             Ctx& wc = (use_lanes && !is_string) ? lane(t, (int)(ci % kLanes)) : t.ctx;
             Buf validity;
             ColumnPtr col;
-            if (max_def > 0) validity = dalloc_zero(t.ctx, bitmap_alloc_bytes(n_rows));
+            if (max_def > 0 || cs.cv.kind == PQ_CV_TS_MUL) validity = dalloc_zero(t.ctx, bitmap_alloc_bytes(n_rows));   // (overflowing products are NULL)
             if (!is_string) {
                 col = std::make_shared<Column>();
                 col->type = fld.type;
@@ -845,6 +940,9 @@ struct ParquetScanExec : Operator, FusedScanSource {
             a.out_type = fld.type.id;
             a.out_width = fld.type.width();
             a.out_unit = fld.type.unit;
+            a.conv = cs.cv.kind;
+            a.conv_mul = cs.cv.mul;
+            a.conv_mul_hi = cs.cv.mul_hi;
             a.max_def = max_def;
             a.out_valid = P<uint32_t>(validity);
             if (is_string) {
@@ -869,8 +967,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
                     col->null_count = -1;
                 }
                 const TypeId ot = fld.type.id;
-                if (cs.stat_ok && cs.stat_min <= cs.stat_max && (ot == T_INT32 || ot == T_INT64 || ot == T_DATE32) && fld.type.width() >= phys_width(el.type, el.type_length) &&
-                    !getenv("AURON_SCAN_NO_STATS")) {
+                if (cs.stat_ok && cs.stat_min <= cs.stat_max && (ot == T_INT32 || ot == T_INT64 || ot == T_DATE32) && !getenv("AURON_SCAN_NO_STATS")) {
                     col->has_range = true;
                     col->range_min = cs.stat_min;
                     col->range_max = cs.stat_max;
@@ -984,7 +1081,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
                     p.cols[ci].leaf = li;
                     if (li < 0) continue;
                     p.cols[ci].el = cur->leaves[li].el;
-                    check_types(p.cols[ci].el, fld.type);
+                    p.cols[ci].cv = conversion_of(p.cols[ci].el, fld.type);
                     p.cols[ci].is_string = p.cols[ci].el.type == pq::PT_BYTE_ARRAY;
                 }
             }
@@ -1290,20 +1387,10 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 cs.has_delta = cs.has_delta || cp.has_delta;
                 cs.needs_decomp = true;
             }
-            {   // statistics -> value bounds (Statistics.min_value / max_value are PLAIN-encoded: little-endian two's complement)
+            {   // statistics -> bounds of the converted values
                 const pq::Statistics& st = ct.cm->stats;
-                const size_t w = cs.el.type == pq::PT_INT32 ? 4 : cs.el.type == pq::PT_INT64 ? 8 : 0;
-                if (w && st.has_min && st.has_max && st.min_value.size() == w && st.max_value.size() == w) {
-                    int64_t mn, mx;
-                    if (w == 4) {
-                        int32_t a, b;
-                        memcpy(&a, st.min_value.data(), 4);
-                        memcpy(&b, st.max_value.data(), 4);
-                        mn = a, mx = b;
-                    } else {
-                        memcpy(&mn, st.min_value.data(), 8);
-                        memcpy(&mx, st.max_value.data(), 8);
-                    }
+                int64_t mn, mx;
+                if (converted_bounds(cs.el, cs.cv, st, &mn, &mx)) {
                     cs.stat_min = std::min(cs.stat_min, mn);
                     cs.stat_max = std::max(cs.stat_max, mx);
                 } else if (!(st.has_null_count && st.null_count == ct.cm->num_values)) {
@@ -1608,7 +1695,8 @@ struct ParquetScanExec : Operator, FusedScanSource {
         for (int c : used) {
             const ColState& cs = p.cols[(size_t)c];
             const DType& ft = proj_field(projection[(size_t)c]).type;
-            if (cs.leaf < 0 || cs.is_string || cs.el.type != pq::PT_INT32 || !fused_type_ok(ft)) return false;
+            // (the fused kernels read INT32 values as signed integers: copies and sign extensions only)
+            if (cs.leaf < 0 || cs.is_string || cs.el.type != pq::PT_INT32 || !fused_type_ok(ft) || (cs.cv.kind != PQ_CV_COPY && cs.cv.kind != PQ_CV_SEXT)) return false;
         }
         // key range of this batch from the column-chunk statistics; the table is widened to the union
         const ColState& kcs = p.cols[(size_t)spec.key_col];
