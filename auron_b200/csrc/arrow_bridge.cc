@@ -57,8 +57,22 @@ std::string format_of(const DType& t) {
             return std::string("ts") + u + ":" + t.tz;
         }
         case T_DECIMAL128: return "d:" + std::to_string(t.precision) + "," + std::to_string(t.scale);
+        case T_LIST: return "+l";
     }
     return "n";
+}
+
+// a field's type from its schema: a list ("+l") takes its element from the one child, which must be flat
+static DType dtype_from_schema(const ArrowSchema* c) {
+    AURON_CHECK(c->dictionary == nullptr, "dictionary-encoded columns are not supported");
+    std::string f(c->format ? c->format : "");
+    if (f == "+L" || f.rfind("+w:", 0) == 0) fail("unsupported Arrow format string '" + f + "': only 32-bit-offset lists are supported");
+    if (f != "+l") return dtype_from_format(c->format);
+    AURON_CHECK(c->n_children == 1 && c->children[0], "malformed Arrow list schema");
+    const ArrowSchema* e = c->children[0];
+    DType et = dtype_from_schema(e);
+    if (et.id == T_LIST) fail("a list whose element is itself a list: nested types are out of scope");
+    return DType::list(et, (e->flags & 2) != 0, e->name ? e->name : "item");
 }
 
 Schema schema_from_arrow(const ArrowSchema* s) {
@@ -69,7 +83,7 @@ Schema schema_from_arrow(const ArrowSchema* s) {
         AURON_CHECK(c->dictionary == nullptr, "dictionary-encoded columns are not supported");
         Field f;
         f.name = c->name ? c->name : "";
-        f.type = dtype_from_format(c->format);
+        f.type = dtype_from_schema(c);
         f.nullable = (c->flags & 2) != 0;
         out.fields.push_back(f);
     }
@@ -101,12 +115,22 @@ static void fill_schema(ArrowSchema* out, const std::string& format, const std::
     out->release = release_schema;
     out->private_data = p;
 }
+static void fill_field_schema(ArrowSchema* c, const DType& t, const std::string& name, bool nullable) {
+    fill_schema(c, format_of(t), name, nullable);
+    if (t.id != T_LIST) return;
+    auto* p = static_cast<SchemaPriv*>(c->private_data);
+    auto* e = new ArrowSchema;
+    fill_field_schema(e, *t.elem, t.elem_name, t.elem_nullable);
+    p->children.push_back(e);
+    c->n_children = 1;
+    c->children = p->children.data();
+}
 void schema_to_arrow(const Schema& s, ArrowSchema* out) {
     fill_schema(out, "+s", "", false);
     auto* p = static_cast<SchemaPriv*>(out->private_data);
     for (auto& f : s.fields) {
         auto* c = new ArrowSchema;
-        fill_schema(c, format_of(f.type), f.name, true);
+        fill_field_schema(c, f.type, f.name, true);
         p->children.push_back(c);
     }
     out->n_children = (int64_t)p->children.size();
@@ -171,6 +195,26 @@ static ColumnPtr import_column(Ctx& ctx, const ArrowArray* a, const DType& t) {
         c->data_bytes = last - first;
         c->data = dalloc(ctx, (size_t)c->data_bytes);
         if (c->data_bytes) CUDA_OK(cudaMemcpyAsync(c->data->ptr, data + first, (size_t)c->data_bytes, cudaMemcpyHostToDevice, ctx.stream));
+    } else if (t.id == T_LIST) {
+        // offsets rebased to start at 0; the child keeps only elements [offsets[off], offsets[off + len]) of its array
+        AURON_CHECK(a->n_buffers >= 2 && a->n_children == 1 && a->children[0], "malformed Arrow list array");
+        const int32_t* offs = static_cast<const int32_t*>(a->buffers[1]);
+        int32_t first = len ? offs[off] : 0, last = len ? offs[off + len] : 0;
+        const ArrowArray* ch = a->children[0];
+        AURON_CHECK(first >= 0 && last >= first && last <= ch->length, "Arrow list offsets outside the child array");
+        std::vector<int32_t> tmp((size_t)len + 1, 0);
+        for (int64_t i = 0; i <= len && len; i++) {
+            tmp[(size_t)i] = offs[off + i] - first;
+            AURON_CHECK(i == 0 || tmp[(size_t)i] >= tmp[(size_t)i - 1], "Arrow list offsets are not monotonic");
+        }
+        c->offsets = dalloc(ctx, (size_t)(len + 1) * 4);
+        CUDA_OK(cudaMemcpyAsync(c->offsets->ptr, tmp.data(), tmp.size() * 4, cudaMemcpyHostToDevice, ctx.stream));
+        ArrowArray view = *ch;   // shallow: same buffers, the window of this slice
+        view.offset += first;
+        view.length = last - first;
+        if (view.null_count != 0) view.null_count = -1;
+        c->child = import_column(ctx, &view, *t.elem);
+        ctx.sync();   // tmp dies here
     } else {
         fail("import: unsupported type " + t.str());
     }
@@ -251,6 +295,7 @@ static size_t export_bytes(const Column& c) {   // upper bound of what export_co
     if (c.type.id == T_BOOL) t += al(bitmap_alloc_bytes(c.len) + 8);
     else if (c.type.width() > 0) t += al(n * (size_t)c.type.width());
     else if (c.type.is_varlen()) t += al((n + 1) * 4) + al((size_t)c.data_bytes);
+    else if (c.type.id == T_LIST) t += al((n + 1) * 4) + export_bytes(*c.child);
     return t;
 }
 static int64_t count_nulls(const uint8_t* bits, int64_t n) {
@@ -296,12 +341,26 @@ static void export_column(Ctx& ctx, const Column& c, ArrowArray* out, const std:
         if (c.data_bytes) CUDA_OK(cudaMemcpyAsync(d, c.data->ptr, (size_t)c.data_bytes, cudaMemcpyDeviceToHost, ctx.stream));
         p->buffers.push_back(o);
         p->buffers.push_back(d);
+    } else if (c.type.id == T_LIST) {
+        int32_t* o = (int32_t*)host_alloc(p, (size_t)(n + 1) * 4);
+        CUDA_OK(cudaMemcpyAsync(o, c.offsets->ptr, (size_t)(n + 1) * 4, cudaMemcpyDeviceToHost, ctx.stream));
+        p->buffers.push_back(o);
+        auto* ch = new ArrowArray;
+        export_column(ctx, *c.child, ch, block);
+        p->children.push_back(ch);
+        out->n_children = 1;
+        out->children = p->children.data();
     } else {
         fail("export: unsupported type " + c.type.str());
     }
     out->null_count = hv ? -1 : 0;   // counted after the batch's single sync
     out->n_buffers = (int64_t)p->buffers.size();
     out->buffers = p->buffers.data();
+}
+
+static void fix_null_counts(ArrowArray* a) {
+    if (a->null_count < 0) a->null_count = count_nulls((const uint8_t*)a->buffers[0], a->length);
+    for (int64_t k = 0; k < a->n_children; k++) fix_null_counts(a->children[k]);
 }
 
 void export_batch(Ctx& ctx, const Batch& b, const Schema& schema, ArrowArray* out, size_t pinned_from) {
@@ -332,10 +391,7 @@ void export_batch(Ctx& ctx, const Batch& b, const Schema& schema, ArrowArray* ou
         p->children.push_back(ch);
     }
     ctx.sync();   // one sync for every buffer of the batch
-    for (size_t i = 0; i < b.cols.size(); i++) {
-        ArrowArray* ch = p->children[i];
-        if (ch->null_count < 0) ch->null_count = count_nulls((const uint8_t*)ch->buffers[0], ch->length);
-    }
+    for (size_t i = 0; i < b.cols.size(); i++) fix_null_counts(p->children[i]);
     out->n_children = (int64_t)p->children.size();
     out->children = p->children.data();
 }

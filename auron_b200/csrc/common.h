@@ -54,6 +54,7 @@ enum TypeId : int32_t {
     T_DATE64 = 11,
     T_TIMESTAMP = 12,  // int64, unit in DType::unit (0 s, 1 ms, 2 us, 3 ns)
     T_DECIMAL128 = 13,
+    T_LIST = 14,       // one level: the element is a flat type (DType::elem); int32 offsets + a child column
 };
 
 struct DType {
@@ -61,6 +62,10 @@ struct DType {
     int32_t precision = 0, scale = 0;  // decimal
     int32_t unit = 2;                  // timestamp unit
     std::string tz;
+    // T_LIST: the element's type, and the name and nullability of the child field (kept for the Arrow export)
+    std::shared_ptr<const DType> elem;
+    std::string elem_name = "item";
+    bool elem_nullable = true;
     DType() = default;
     DType(TypeId i) : id(i) {}
     static DType decimal(int p, int s) {
@@ -69,10 +74,18 @@ struct DType {
         t.scale = s;
         return t;
     }
+    static DType list(const DType& e, bool nullable = true, const std::string& name = "item") {
+        DType t(T_LIST);
+        t.elem = std::make_shared<const DType>(e);
+        t.elem_nullable = nullable;
+        t.elem_name = name;
+        return t;
+    }
     bool operator==(const DType& o) const {
         if (id != o.id) return false;
         if (id == T_DECIMAL128) return precision == o.precision && scale == o.scale;
         if (id == T_TIMESTAMP) return unit == o.unit;
+        if (id == T_LIST) return elem && o.elem && *elem == *o.elem;
         return true;
     }
     bool operator!=(const DType& o) const { return !(*this == o); }
@@ -193,12 +206,14 @@ struct Column {
     int64_t null_count = 0;
     Buf validity;  // bitmap, bit i of byte i/8 (LSB first); nullptr => all valid
     Buf data;      // values; bool => bitmap; utf8/binary => bytes
-    Buf offsets;   // int32[len+1] for utf8/binary
+    Buf offsets;   // int32[len+1] for utf8/binary and list
     int64_t data_bytes = 0;  // utf8/binary: number of payload bytes (== offsets[len])
     // optional bounds of the non-null values of an integer column (a superset is fine): set by the Parquet scan from the
     // column-chunk statistics, used by the aggregate's direct-address path instead of a min/max pass over the keys
     bool has_range = false;
     int64_t range_min = 0, range_max = 0;
+    // list: the elements of every row, row i owning child rows [offsets[i], offsets[i+1]) (offsets[0] == 0)
+    std::shared_ptr<Column> child;
 
     const uint8_t* vbits() const { return validity ? static_cast<const uint8_t*>(validity->ptr) : nullptr; }
     bool may_have_nulls() const { return validity != nullptr; }

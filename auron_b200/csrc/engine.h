@@ -110,7 +110,12 @@ struct HostArray {
     std::vector<uint8_t> validity;   // empty = no nulls
     std::vector<uint8_t> data;       // values (bool: bitmap; utf8/binary: bytes)
     std::vector<int32_t> offsets;    // utf8/binary
+    // the list row itself (list literals): NULL, and the name / nullability of its element field
+    bool list_is_null = false;
+    std::string elem_name = "item";
+    bool elem_nullable = true;
 };
+bool is_list_scalar_ipc(const uint8_t* bytes, size_t n);   // a ScalarValue whose type is List
 HostArray decode_list_scalar_ipc(const uint8_t* bytes, size_t n);
 ColumnPtr host_array_to_device(Ctx& ctx, const HostArray& a);
 

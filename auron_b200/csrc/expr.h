@@ -40,6 +40,7 @@ enum ExprKind {
     E_ROW_NUM,     // RowNumExprNode: int64 position of the row among the rows the projection emitted (row_num.rs)
 };
 
+struct HostArray;   // engine.h
 struct Expr;
 using ExprPtr = std::shared_ptr<Expr>;
 struct Expr {
@@ -50,6 +51,7 @@ struct Expr {
     std::string op;     // binary operator
     Literal lit;
     DType type;         // cast target / function return type
+    std::shared_ptr<const HostArray> list_lit;   // E_LITERAL of a list type: the elements of the one list row (lit.is_null: NULL list)
     bool negated = false, case_insensitive = false, has_case_expr = false, has_else = false;
 };
 
@@ -63,6 +65,11 @@ DType infer_type(const Expr& e, const Schema& input);
 bool makes_string_fn(const std::string& name);
 // true when the expression is a bare column reference; *idx receives the resolved index
 bool is_plain_column(const Expr& e, const Schema& input, int* idx);
+// list values (list columns, list literals, Spark_StringSplit, Spark_MakeArray) are computed outside the VM, only as a whole
+// projection expression or a generator's child (operators.cc ListExpr); the compilers reject them anywhere inside a program
+bool is_list_fn(const std::string& name);
+// keys evaluated only when the plan runs (sort, join, window, shuffle): rejected when the plan is built if a list value is among them
+void reject_list_exprs(const std::vector<ExprPtr>& exprs, const Schema& input, const char* where);
 
 // ---- compiled program -------------------------------------------------------------------
 struct VmProgramImpl;

@@ -29,6 +29,7 @@ std::string DType::str() const {
         case T_DATE64: return "date64";
         case T_TIMESTAMP: return "timestamp";
         case T_DECIMAL128: return "decimal128(" + std::to_string(precision) + "," + std::to_string(scale) + ")";
+        case T_LIST: return "list<" + (elem ? elem->str() : std::string("?")) + ">";
     }
     return "?";
 }
@@ -557,6 +558,42 @@ __global__ void __launch_bounds__(256) take_bytes_kernel(const int32_t* __restri
     for (int32_t k = 0; k < len; k++) d[k] = s[k];
 }
 
+// list rows: the element count of row idx[i]; a NULL row counts as empty (Arrow lets it cover a range of the child)
+__global__ void __launch_bounds__(256) list_lens_kernel(const int32_t* __restrict__ in_off, const uint8_t* __restrict__ in_valid,
+                                                        const int32_t* __restrict__ idx, int64_t n_out, int64_t* __restrict__ lens,
+                                                        uint32_t* __restrict__ out_valid) {
+    int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    bool ok = false;
+    if (i < n_out) {
+        int64_t src = idx ? (int64_t)idx[i] : i;
+        ok = src >= 0 && valid_at(in_valid, src);
+        lens[i] = ok ? (int64_t)(in_off[src + 1] - in_off[src]) : 0;
+    }
+    if (out_valid) {
+        uint32_t word = __ballot_sync(FULL_MASK, ok);
+        if (lane_id() == 0 && i < n_out) out_valid[i >> 5] = word;
+    }
+}
+// row of output element j: the last i with out_off[i] <= j among rows that own elements
+__device__ __forceinline__ int64_t row_of_offset(const int32_t* __restrict__ off, int64_t n, int64_t j) {
+    int64_t lo = 0, hi = n;   // off[lo] <= j < off[hi]
+    while (hi - lo > 1) {
+        int64_t mid = (lo + hi) >> 1;
+        if ((int64_t)off[mid] <= j) lo = mid;
+        else hi = mid;
+    }
+    return lo;
+}
+__global__ void __launch_bounds__(256) list_elem_index_kernel(const int32_t* __restrict__ in_off, const int32_t* __restrict__ idx,
+                                                              const int32_t* __restrict__ out_off, int64_t n_out, int64_t total,
+                                                              int32_t* __restrict__ eidx) {
+    int64_t j = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    if (j >= total) return;
+    int64_t i = row_of_offset(out_off, n_out, j);
+    int64_t src = idx ? (int64_t)idx[i] : i;
+    eidx[j] = in_off[src] + (int32_t)(j - out_off[i]);
+}
+
 struct alignas(16) u128_t {
     uint64_t a, b;
 };
@@ -619,6 +656,29 @@ ColumnPtr take(Ctx& ctx, const Column& in, const int32_t* idx, int64_t n_out, bo
             take_bytes_kernel<<<blocks, 256, 0, ctx.stream>>>(P<int32_t>(in.offsets), P<uint8_t>(in.data), idx, n_out, P<int32_t>(out->offsets), P<uint8_t>(out->data));
             LAUNCH_CHECK(ctx);
         }
+    } else if (in.type.id == T_LIST) {
+        out->offsets = dalloc(ctx, (size_t)(n_out + 1) * 4);
+        int64_t total = 0;
+        Buf lens = dalloc(ctx, (size_t)(n_out + 1) * 8);
+        if (blocks) {
+            list_lens_kernel<<<blocks, 256, 0, ctx.stream>>>(P<int32_t>(in.offsets), in.vbits(), idx, n_out, P<int64_t>(lens), ov);
+            LAUNCH_CHECK(ctx);
+            exclusive_scan_i64(ctx, P<int64_t>(lens), P<int64_t>(lens), n_out, P<int64_t>(lens) + n_out);
+            narrow_offsets_kernel<<<(unsigned)((n_out + 1 + 255) / 256), 256, 0, ctx.stream>>>(P<int64_t>(lens), P<int32_t>(out->offsets), n_out + 1);
+            LAUNCH_CHECK(ctx);
+            to_host(ctx, &total, P<int64_t>(lens) + n_out, 8);
+            AURON_CHECK(total <= (int64_t)INT32_MAX, "list column of " + std::to_string(total) + " elements exceeds 2^31 - 1 elements in one batch");
+        } else {
+            CUDA_OK(cudaMemsetAsync(out->offsets->ptr, 0, 4, ctx.stream));
+        }
+        // the element each output element copies: one thread per output element finds its row by a search over the new offsets
+        Buf eidx = dalloc(ctx, (size_t)std::max<int64_t>(total, 1) * 4);
+        if (total > 0) {
+            list_elem_index_kernel<<<(unsigned)((total + 255) / 256), 256, 0, ctx.stream>>>(P<int32_t>(in.offsets), idx, P<int32_t>(out->offsets), n_out,
+                                                                                            total, P<int32_t>(eidx));
+            LAUNCH_CHECK(ctx);
+        }
+        out->child = take(ctx, *in.child, P<int32_t>(eidx), total, false);
     } else {
         fail("take: unsupported type " + in.type.str());
     }
@@ -662,6 +722,16 @@ ColumnPtr concat_columns(Ctx& ctx, const std::vector<ColumnPtr>& cols) {
         out->offsets = dalloc(ctx, (size_t)(total + 1) * 4);
         out->data = dalloc(ctx, (size_t)total_bytes);
         out->data_bytes = total_bytes;
+    } else if (out->type.id == T_LIST) {
+        int64_t elems = 0;
+        std::vector<ColumnPtr> kids;
+        for (auto& c : cols) {
+            elems += c->child->len;
+            kids.push_back(c->child);
+        }
+        AURON_CHECK(elems <= (int64_t)INT32_MAX, "list column of " + std::to_string(elems) + " elements exceeds 2^31 - 1 elements in one batch");
+        out->offsets = dalloc(ctx, (size_t)(total + 1) * 4);
+        out->child = concat_columns(ctx, kids);
     }
     int64_t row = 0, byte = 0;
     for (auto& c : cols) {
@@ -680,10 +750,15 @@ ColumnPtr concat_columns(Ctx& ctx, const std::vector<ColumnPtr>& cols) {
             if (c->data_bytes)
                 CUDA_OK(cudaMemcpyAsync(P<uint8_t>(out->data) + byte, c->data->ptr, (size_t)c->data_bytes, cudaMemcpyDeviceToDevice, ctx.stream));
             byte += c->data_bytes;
+        } else if (out->type.id == T_LIST) {
+            rebase_offsets_kernel<<<(unsigned)((c->len + 1 + 255) / 256), 256, 0, ctx.stream>>>(P<int32_t>(c->offsets), c->len + 1, (int32_t)byte,
+                                                                                              P<int32_t>(out->offsets) + row);
+            LAUNCH_CHECK(ctx);
+            byte += c->child->len;
         }
         row += c->len;
     }
-    if (out->type.is_varlen() && total == 0) CUDA_OK(cudaMemsetAsync(out->offsets->ptr, 0, 4, ctx.stream));
+    if ((out->type.is_varlen() || out->type.id == T_LIST) && total == 0) CUDA_OK(cudaMemsetAsync(out->offsets->ptr, 0, 4, ctx.stream));
     return out;
 }
 

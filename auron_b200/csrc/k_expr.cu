@@ -2188,6 +2188,53 @@ static DType dec_arith_type(const std::string& op, DType a, DType b) {
     return DType::decimal(std::min(38, std::max(a.precision, b.precision) + 1), a.scale);
 }
 
+bool is_list_fn(const std::string& f) { return f == "Spark_StringSplit" || f == "Spark_MakeArray"; }
+
+// a list value at this node: a list column, a list literal, split / array, or a cast to a list type (never resolves a column that
+// does not exist: that error belongs to the compiler)
+static bool is_list_value(const Expr& e, const Schema& in) {
+    if (e.kind == E_COLUMN) {
+        if (e.index >= 0) return e.index < (int)in.fields.size() && in.fields[(size_t)e.index].type.id == T_LIST;
+        const int i = in.index_of(e.name);
+        return i >= 0 && in.fields[(size_t)i].type.id == T_LIST;
+    }
+    if (e.kind == E_LITERAL || e.kind == E_CAST || e.kind == E_TRY_CAST) return (e.kind == E_LITERAL ? e.lit.type : e.type).id == T_LIST;
+    return e.kind == E_SCALAR_FN && (is_list_fn(e.name) || e.type.id == T_LIST);
+}
+static std::string list_value_name(const Expr& e) {
+    if (e.kind == E_COLUMN) return e.index >= 0 ? "list column #" + std::to_string(e.index) : "list column " + e.name;
+    if (e.kind == E_LITERAL) return "list literal";
+    if (e.kind == E_SCALAR_FN) return e.name;
+    return e.kind == E_CAST ? "CAST to a list" : "TRY_CAST to a list";
+}
+static std::string node_name(const Expr& e) {
+    switch (e.kind) {
+        case E_SCALAR_FN: return e.name;
+        case E_CASE: return "CASE";
+        case E_CAST: return "CAST";
+        case E_TRY_CAST: return "TRY_CAST";
+        case E_BINARY: return e.op;
+        case E_IN_LIST: return "IN";
+        case E_LIKE: return "LIKE";
+        case E_IS_NULL: return "IS NULL";
+        case E_IS_NOT_NULL: return "IS NOT NULL";
+        default: return "an expression";
+    }
+}
+// the VM has no list registers: a list value anywhere in a program is a plan error that names it and where it was used
+static void reject_list_values(const Expr& e, const Schema& in, const Expr* parent, const char* where) {
+    if (is_list_value(e, in))
+        fail(list_value_name(e) + (parent ? " inside " + node_name(*parent) : std::string(" as ") + where) +
+             " is not supported: a list value may only be a whole projection expression or a generator's child");
+    for (auto& c : e.children)
+        if (c) reject_list_values(*c, in, &e, where);
+}
+
+void reject_list_exprs(const std::vector<ExprPtr>& exprs, const Schema& input, const char* where) {
+    for (auto& e : exprs)
+        if (e) reject_list_values(*e, input, nullptr, where);
+}
+
 DType infer_type(const Expr& e, const Schema& in) {
     switch (e.kind) {
         case E_COLUMN: return in.fields[resolve_col(e, in)].type;
@@ -2210,6 +2257,9 @@ DType infer_type(const Expr& e, const Schema& in) {
         case E_CAST: case E_TRY_CAST: return e.type;
         case E_SCALAR_FN:
             if (makes_string(e)) return DType(T_UTF8);
+            if (e.name == "Spark_StringSplit") return DType::list(DType(T_UTF8), true, e.type.id == T_LIST ? e.type.elem_name : "item");
+            if (e.name == "Spark_MakeArray" && !e.children.empty())
+                return DType::list(infer_type(*e.children[0], in), true, e.type.id == T_LIST ? e.type.elem_name : "item");
             if (e.type.id != T_NULL) return e.type;
             return infer_type(*e.children[0], in);
     }
@@ -3023,6 +3073,7 @@ VmProgram compile_projection(const std::vector<ExprPtr>& exprs, const Schema& in
     Compiler c(input, *p.impl);
     c.row_num_ok = row_num;
     AURON_CHECK(exprs.size() <= VM_MAX_COLS, "too many projection expressions for one program");
+    for (auto& e : exprs) reject_list_values(*e, input, nullptr, "a computed value (a key or argument of an aggregate, sort, join, window or shuffle)");
     for (size_t i = 0; i < exprs.size(); i++) {
         const Expr& ex = strip_utf8_cast(*exprs[i]);
         const int alg = ex.kind == E_SCALAR_FN ? digest_alg_of(ex.name) : 0;
@@ -3156,6 +3207,7 @@ VmProgram compile_predicate(const std::vector<ExprPtr>& conjuncts, const Schema&
     VmProgram p;
     p.impl = std::make_shared<VmProgramImpl>();
     p.is_predicate = true;
+    for (auto& e : conjuncts) reject_list_values(*e, input, nullptr, "a predicate");
     if (!getenv("AURON_DISABLE_SIMPLE_PREDICATE") && try_compile_simple(conjuncts, input, *p.impl)) return p;
     Compiler c(input, *p.impl);
     AURON_CHECK(!conjuncts.empty(), "empty predicate");

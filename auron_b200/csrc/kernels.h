@@ -29,6 +29,27 @@ BatchPtr concat_batches(Ctx& ctx, const std::vector<BatchPtr>& batches);
 ColumnPtr slice_column(Ctx& ctx, const Column& in, int64_t off, int64_t len);
 BatchPtr slice_batch(Ctx& ctx, const Batch& in, int64_t off, int64_t len);
 
+// ----------------------------------------------------------------------------- k_list.cu
+// Spark_StringSplit (spark_strings.rs:93-115): the pieces of each utf8 row between the leftmost non-overlapping matches of a
+// non-empty pattern; a NULL row gives a NULL list
+ColumnPtr string_split(Ctx& ctx, const Column& s, const std::string& pattern, const DType& out_type);
+// Spark_MakeArray: row i = [args[0][i], ..., args[k-1][i]] (never NULL)
+ColumnPtr make_array(Ctx& ctx, const std::vector<ColumnPtr>& args, int64_t n, const DType& out_type);
+// the one list `elems` (NULL: is_null) in each of n rows
+ColumnPtr broadcast_list(Ctx& ctx, const ColumnPtr& elems, bool is_null, int64_t n, const DType& out_type);
+// explode / posexplode of a list column over n selected rows (row s of the list is input row sel[s]; sel == nullptr: s):
+// rows_cum / bytes_cum = exclusive scans [n + 1] of the output rows per input row and of the bytes they copy of var_cols
+constexpr int kMaxExplodeVarCols = 32;
+void explode_scan(Ctx& ctx, const Column& list, bool outer, const std::vector<ColumnPtr>& var_cols, const int32_t* sel, int64_t n, Buf* rows_cum,
+                  Buf* bytes_cum);
+// end r1 of the piece that starts at selected row r0: the most rows within both limits, at least one (synchronises)
+int64_t explode_cut(Ctx& ctx, const Buf& rows_cum, const Buf& bytes_cum, int64_t n, int64_t r0, int64_t max_rows, int64_t max_bytes, int64_t* out_rows,
+                    int64_t* out_bytes);
+// the n_out output rows of piece [r0, r1): input row, list element (-1 = the NULL row of outer) and, when pos != nullptr, the
+// position (NULL in the outer row)
+void explode_map(Ctx& ctx, const Column& list, const int32_t* sel, const Buf& rows_cum, int64_t r0, int64_t r1, int64_t n_out, int32_t* row_idx,
+                 int32_t* elem_idx, int32_t* pos, uint32_t* pos_valid);
+
 // ----------------------------------------------------------------------------- k_hash.cu
 // Spark-compatible chained column hashing (spark_hash.rs:28-57). kind 0 murmur3 -> int32 out, 1 xxhash64 -> int64 out
 Buf hash_columns(Ctx& ctx, const std::vector<ColumnPtr>& cols, int64_t n, int kind, int64_t seed);

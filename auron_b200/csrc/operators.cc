@@ -42,6 +42,7 @@ std::string json_quote(const std::string& s) {
 }
 static std::string lit_to_string(const Literal& l) {
     if (l.is_null) return "lit(" + l.type.str() + ":NULL)";
+    if (l.type.id == T_LIST) return "lit(" + l.type.str() + ")";
     std::string v;
     switch (l.type.id) {
         case T_FLOAT32: case T_FLOAT64: {
@@ -105,6 +106,14 @@ static std::string exprs_json(const std::vector<ExprPtr>& es) {
 std::string FFIReaderExec::describe() const { return "\"resource_id\":" + json_quote(resource_id); }
 std::string FilterExec::describe() const { return "\"predicates\":" + exprs_json(predicates); }
 std::string ProjectExec::describe() const { return "\"exprs\":" + exprs_json(exprs); }
+std::string GenerateExec::describe() const {
+    std::string o = std::string("\"function\":\"") + (func == GEN_POS_EXPLODE ? "PosExplode" : "Explode") + "\",\"outer\":" + (outer ? "true" : "false") +
+                    ",\"child\":" + json_quote(gen.text) + ",\"required\":[";
+    for (size_t i = 0; i < required_names.size(); i++) o += (i ? "," : "") + json_quote(required_names[i]);
+    o += "],\"generator_output\":[";
+    for (size_t i = 0; i < gen_fields.size(); i++) o += std::string(i ? "," : "") + "[" + json_quote(gen_fields[i].name) + "," + json_quote(gen_fields[i].type.str()) + "]";
+    return o + "]";
+}
 std::string AggExec::describe() const {
     static const char* fn_names[] = {"MIN", "MAX", "SUM", "AVG", "COUNT", "?", "?", "FIRST", "FIRST_IGNORES_NULL"};
     static const char* mode_names[] = {"PARTIAL", "PARTIAL_MERGE", "FINAL"};
@@ -266,6 +275,25 @@ ProjectExec::ProjectExec(OperatorPtr input, std::vector<ExprPtr> ex, std::vector
     for (size_t i = 0; i < exprs.size(); i++) {
         DType actual = infer_type(*exprs[i], in);
         DType declared = i < types.size() && types[i].id != T_NULL ? types[i] : actual;
+        const std::string fname = i < names.size() ? names[i] : ("c" + std::to_string(i));
+        if (actual.id == T_LIST || declared.id == T_LIST) {   // a list value: a bare column, or computed after the VM
+            if (actual != declared) fail("ProjectExec: " + fname + " is " + actual.str() + " but declared " + declared.str() + ": a cast of a list is not supported");
+            int idx = -1;
+            ListExpr le;
+            if (is_plain_column(*exprs[i], in, &idx)) {
+                plain_col.push_back(idx);
+                list_slot.push_back(-1);
+            } else {
+                plan_list_expr(exprs[i], in, declared, &le, &computed);
+                plain_col.push_back(-1);
+                list_slot.push_back((int)lists.size());
+                lists.push_back(std::move(le));
+            }
+            prog_slot.push_back(-1);
+            out_schema.fields.push_back(Field{fname, declared, true});
+            continue;
+        }
+        list_slot.push_back(-1);
         if (actual != declared) {   // planner.rs:145-149 wraps a TryCastExpr when the declared type differs
             auto c = std::make_shared<Expr>();
             c->kind = E_TRY_CAST;
@@ -283,7 +311,7 @@ ProjectExec::ProjectExec(OperatorPtr input, std::vector<ExprPtr> ex, std::vector
             computed.push_back(exprs[i]);
         }
         Field f;
-        f.name = i < names.size() ? names[i] : ("c" + std::to_string(i));
+        f.name = fname;
         f.type = declared;
         out_schema.fields.push_back(f);
     }
@@ -306,12 +334,167 @@ BatchPtr ProjectExec::next(Task& t) {
         if (plain_col[i] >= 0) {
             const ColumnPtr& c = s.batch->cols[plain_col[i]];
             out->cols.push_back(s.sel ? take(t.ctx, *c, P<int32_t>(s.sel), s.n, false) : c);
+        } else if (list_slot[i] >= 0) {
+            out->cols.push_back(eval_list_expr(t, lists[(size_t)list_slot[i]], *s.batch, P<int32_t>(s.sel), s.n, computed));
         } else {
             out->cols.push_back(computed[prog_slot[i]]);
         }
     }
     metrics.add("output_rows", s.n);
     return out;
+}
+
+// ------------------------------------------------------------------------------------------ list expressions
+bool plan_list_expr(const ExprPtr& e, const Schema& in, const DType& declared, ListExpr* out, std::vector<ExprPtr>* args) {
+    const DType actual = infer_type(*e, in);
+    if (actual.id != T_LIST) return false;
+    out->type = declared.id == T_LIST ? declared : actual;
+    out->text = expr_to_string(*e);
+    int idx = -1;
+    if (is_plain_column(*e, in, &idx)) {
+        out->kind = ListExpr::COLUMN;
+        out->col = idx;
+        return true;
+    }
+    if (e->kind == E_LITERAL) {
+        out->kind = ListExpr::LITERAL;
+        out->lit = e->list_lit;
+        AURON_CHECK(out->lit != nullptr, "list literal without its elements");
+        return true;
+    }
+    if (e->kind == E_SCALAR_FN && e->name == "Spark_StringSplit") {   // spark_strings.rs:93-115 (ShimsImpl: split(s, <literal>))
+        if (e->children.size() != 2) fail("Spark_StringSplit takes a string and a pattern");
+        const Expr& pat = *e->children[1];
+        if (pat.kind != E_LITERAL || pat.lit.type.id != T_UTF8 || pat.lit.is_null || pat.lit.s.empty())
+            fail("Spark_StringSplit: the pattern must be a non-empty utf8 literal, got " + expr_to_string(pat));
+        const DType st = infer_type(*e->children[0], in);
+        if (st.id != T_UTF8) fail("Spark_StringSplit needs a utf8 string, got " + st.str());
+        out->kind = ListExpr::SPLIT;
+        out->pattern = pat.lit.s;
+        out->arg_slots.push_back((int)args->size());
+        args->push_back(e->children[0]);
+        return true;
+    }
+    if (e->kind == E_SCALAR_FN && e->name == "Spark_MakeArray") {   // spark_make_array.rs
+        if (e->children.empty()) fail("Spark_MakeArray needs at least one argument");
+        const DType et = infer_type(*e->children[0], in);
+        for (auto& c : e->children) {
+            const DType ct = infer_type(*c, in);
+            if (ct != et || ct.id == T_NULL || ct.id == T_LIST)
+                fail("Spark_MakeArray: every argument must have one flat type, got " + et.str() + " and " + ct.str());
+        }
+        out->kind = ListExpr::MAKE_ARRAY;
+        for (auto& c : e->children) {
+            out->arg_slots.push_back((int)args->size());
+            args->push_back(c);
+        }
+        return true;
+    }
+    fail(expr_to_string(*e) + ": this list expression is not native on device (only list columns, list literals, Spark_StringSplit and Spark_MakeArray)");
+}
+ColumnPtr eval_list_expr(Task& t, ListExpr& le, const Batch& b, const int32_t* sel, int64_t n, const std::vector<ColumnPtr>& computed) {
+    switch (le.kind) {
+        case ListExpr::COLUMN: {
+            const ColumnPtr& c = b.cols[(size_t)le.col];
+            return sel ? take(t.ctx, *c, sel, n, false) : c;
+        }
+        case ListExpr::LITERAL:
+            if (!le.lit_dev) le.lit_dev = host_array_to_device(t.ctx, *le.lit);
+            return broadcast_list(t.ctx, le.lit_dev, le.lit->list_is_null, n, le.type);
+        case ListExpr::SPLIT: return string_split(t.ctx, *computed[(size_t)le.arg_slots[0]], le.pattern, le.type);
+        case ListExpr::MAKE_ARRAY: {
+            std::vector<ColumnPtr> args;
+            for (int k : le.arg_slots) args.push_back(computed[(size_t)k]);
+            return make_array(t.ctx, args, n, le.type);
+        }
+    }
+    fail("unknown list expression");
+}
+
+// ------------------------------------------------------------------------------------------ GenerateExec
+GenerateExec::GenerateExec(OperatorPtr input, int fn, const ExprPtr& child, std::vector<std::string> req, std::vector<Field> gen_output, bool out)
+    : func(fn), outer(out), required_names(std::move(req)), gen_fields(std::move(gen_output)) {
+    name = "GenerateExec";
+    const Schema& in = input->out_schema;
+    const char* fname = func == GEN_POS_EXPLODE ? "PosExplode" : "Explode";
+    std::vector<ExprPtr> args;
+    const DType ct = infer_type(*child, in);
+    if (ct.id != T_LIST) fail(std::string(fname) + " of a " + ct.str() + " value is not native in auron_b200 (only lists are exploded)");
+    plan_list_expr(child, in, ct, &gen, &args);
+    if (!args.empty()) {
+        prog = compile_projection(args, in);
+        has_prog = true;
+    }
+    for (auto& nm : required_names) {   // planner.rs:790-795: resolved by name
+        const int i = in.index_of(nm);
+        if (i < 0) fail("GenerateExec: required child column " + nm + " is not in the input schema");
+        required.push_back(i);
+        out_schema.fields.push_back(in.fields[(size_t)i]);
+    }
+    // generator output: [pos int32,] element, of exactly the types the generator produces (Spark always sends them so)
+    const size_t want = func == GEN_POS_EXPLODE ? 2 : 1;
+    if (gen_fields.size() != want) fail(std::string("GenerateExec: ") + fname + " produces " + std::to_string(want) + " columns, the plan declares " + std::to_string(gen_fields.size()));
+    if (func == GEN_POS_EXPLODE && gen_fields[0].type != DType(T_INT32))
+        fail("GenerateExec: PosExplode's position column " + gen_fields[0].name + " must be int32, the plan declares " + gen_fields[0].type.str());
+    const Field& ef = gen_fields.back();
+    if (ef.type != *gen.type.elem)
+        fail("GenerateExec: " + std::string(fname) + "'s value column " + ef.name + " must be " + gen.type.elem->str() + ", the plan declares " + ef.type.str());
+    for (auto& f : gen_fields) out_schema.fields.push_back(f);
+    children.push_back(std::move(input));
+}
+BatchPtr GenerateExec::next(Task& t) {
+    for (;;) {
+        if (!cur.batch || next_row >= cur.n) {
+            cur = children[0]->next_sel(t);
+            if (!cur.batch) return nullptr;
+            OpTimer timer(metrics, "elapsed_compute");
+            const int32_t* sel = ensure_sel(t, cur);
+            std::vector<ColumnPtr> computed;
+            if (has_prog) computed = eval_projection(t.ctx, prog, *cur.batch, sel, cur.n);
+            list = eval_list_expr(t, gen, *cur.batch, sel, cur.n, computed);
+            std::vector<ColumnPtr> var;
+            for (int c : required)
+                if (cur.batch->cols[(size_t)c]->type.is_varlen()) var.push_back(cur.batch->cols[(size_t)c]);
+            explode_scan(t.ctx, *list, outer, var, sel, cur.n, &rows_cum, &bytes_cum);
+            next_row = 0;
+            if (cur.n == 0) continue;
+        }
+        OpTimer timer(metrics, "elapsed_compute");
+        const int64_t r0 = next_row;
+        int64_t rows = 0, bytes = 0;
+        const int64_t r1 = explode_cut(t.ctx, rows_cum, bytes_cum, cur.n, r0, t.ctx.gpu_chunk_rows, (int64_t)INT32_MAX, &rows, &bytes);
+        next_row = r1;
+        if (bytes > (int64_t)INT32_MAX)
+            fail("GenerateExec: input row " + std::to_string(r0) + " explodes into " + std::to_string(bytes) +
+                 " bytes of required string columns, more than int32 offsets address in one batch");
+        if (rows > (int64_t)INT32_MAX) fail("GenerateExec: input row " + std::to_string(r0) + " explodes into more than 2^31 - 1 rows");
+        if (rows == 0) continue;
+        const int32_t* sel = P<int32_t>(cur.sel);
+        Buf row_idx = dalloc(t.ctx, (size_t)rows * 4), elem_idx = dalloc(t.ctx, (size_t)rows * 4);
+        Buf pos, pos_valid;
+        if (func == GEN_POS_EXPLODE) {
+            pos = dalloc(t.ctx, (size_t)rows * 4);
+            if (outer) pos_valid = dalloc(t.ctx, bitmap_alloc_bytes(rows));
+        }
+        explode_map(t.ctx, *list, sel, rows_cum, r0, r1, rows, P<int32_t>(row_idx), P<int32_t>(elem_idx), P<int32_t>(pos), P<uint32_t>(pos_valid));
+        auto out = std::make_shared<Batch>();
+        out->num_rows = rows;
+        for (int c : required) out->cols.push_back(take(t.ctx, *cur.batch->cols[(size_t)c], P<int32_t>(row_idx), rows, false));
+        if (func == GEN_POS_EXPLODE) {
+            auto pc = std::make_shared<Column>();
+            pc->type = DType(T_INT32);
+            pc->len = rows;
+            pc->data = pos;
+            if (pos_valid) {
+                pc->validity = pos_valid;
+                pc->null_count = -1;
+            }
+            out->cols.push_back(pc);
+        }
+        out->cols.push_back(take(t.ctx, *list->child, P<int32_t>(elem_idx), rows, outer));
+        metrics.add("output_rows", rows);
+        return out;
+    }
 }
 
 // ------------------------------------------------------------------------------------------ ExpandExec

@@ -67,11 +67,31 @@ struct FilterExec : Operator {
     SelBatch apply(Task& t, const BatchPtr& b);   // the predicates over one batch
 };
 
+// A list-valued expression, computed outside the expression VM: a list column, a list literal, or Spark_StringSplit /
+// Spark_MakeArray over flat arguments the VM computes.  Valid only as a whole projection expression or a generator's child.
+struct ListExpr {
+    enum Kind { COLUMN, LITERAL, SPLIT, MAKE_ARRAY } kind = COLUMN;
+    DType type;                                  // the declared list type (its element field names the exported child)
+    int col = -1;                                // COLUMN: input column
+    std::vector<int> arg_slots;                  // SPLIT: the string, MAKE_ARRAY: the elements, as outputs of the caller's VM program
+    std::string pattern;                         // SPLIT
+    std::shared_ptr<const HostArray> lit;        // LITERAL: its elements (HostArray::list_is_null: the NULL list)
+    ColumnPtr lit_dev;                           // LITERAL: the elements uploaded once
+    std::string text;                            // the expression, for explain
+};
+// `e` as a ListExpr (its flat arguments appended to *args); false when `e` is not list-valued.  Rejects, naming the function,
+// a list expression this engine does not compute.
+bool plan_list_expr(const ExprPtr& e, const Schema& in, const DType& declared, ListExpr* out, std::vector<ExprPtr>* args);
+// the list column of the n rows sel[0..n) (sel == nullptr: 0..n) of `b`; `computed` holds the program outputs over those rows
+ColumnPtr eval_list_expr(Task& t, ListExpr& le, const Batch& b, const int32_t* sel, int64_t n, const std::vector<ColumnPtr>& computed);
+
 // project_exec.rs:135-232 (fuses with a FilterExec child through next_sel)
 struct ProjectExec : Operator {
     std::vector<ExprPtr> exprs;
     std::vector<int> plain_col;       // >= 0: bare column index, -1: computed
     std::vector<int> prog_slot;       // index into the VM program outputs for computed exprs
+    std::vector<int> list_slot;       // >= 0: index into `lists` for list-valued exprs
+    std::vector<ListExpr> lists;
     VmProgram prog;
     bool has_prog = false;
     int64_t rows_out = 0;             // rows emitted so far: the base of RowNum
@@ -296,6 +316,29 @@ struct ExpandExec : Operator {
     BatchPtr cur;
     size_t next_proj = 0;
     ExpandExec(OperatorPtr input, const Schema& schema, std::vector<std::vector<ExprPtr>> projections);
+    std::string describe() const override;
+    BatchPtr next(Task& t) override;
+};
+
+// generate_exec.rs:120-310 + generate/explode.rs: explode / posexplode of a list column, with or without `outer`.  The input comes
+// through next_sel (a Filter below hands over its selection); the output of one input batch is cut between input rows into
+// pieces of at most gpu_chunk_rows rows whose string columns stay addressable with int32 offsets.
+enum GenerateFn { GEN_EXPLODE = 0, GEN_POS_EXPLODE = 1 };
+struct GenerateExec : Operator {
+    int func = GEN_EXPLODE;
+    bool outer = false;
+    std::vector<int> required;            // input columns copied once per output row
+    std::vector<std::string> required_names;
+    std::vector<Field> gen_fields;        // [pos int32,] element
+    ListExpr gen;
+    VmProgram prog;                       // flat arguments of gen
+    bool has_prog = false;
+    // the input batch being exploded (one at a time)
+    SelBatch cur;
+    ColumnPtr list;
+    Buf rows_cum, bytes_cum;
+    int64_t next_row = 0;
+    GenerateExec(OperatorPtr input, int func, const ExprPtr& child, std::vector<std::string> required, std::vector<Field> gen_output, bool outer);
     std::string describe() const override;
     BatchPtr next(Task& t) override;
 };

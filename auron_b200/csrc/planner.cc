@@ -8,6 +8,7 @@
 namespace auron {
 
 // ------------------------------------------------------------------------------------------ types
+static Field decode_field(const uint8_t* b, size_t n);
 DType decode_arrow_type(const uint8_t* b, size_t n) {
     PbReader r(b, n);
     uint32_t f, w;
@@ -57,7 +58,26 @@ DType decode_arrow_type(const uint8_t* b, size_t n) {
                 break;
             }
             case 3: case 5: case 7: case 9: fail("unsigned integer columns are not supported on device");
-            case 25: case 26: case 27: fail("unsupported ArrowType list (tag " + std::to_string(f) + "): nested types are out of scope");
+            case 25: {   // List{field_type=1}: one level of a flat element type
+                Field e;
+                PbReader lr(sb, sn);
+                uint32_t lf, lw;
+                bool has = false;
+                while (lr.next(&lf, &lw)) {
+                    if (lf == 1 && lw == 2) {
+                        const uint8_t* eb;
+                        size_t en;
+                        lr.bytes_view(&eb, &en);
+                        e = decode_field(eb, en);
+                        has = true;
+                    } else lr.skip(lw);
+                }
+                AURON_CHECK(has, "ArrowType list without its element field");
+                if (e.type.id == T_LIST) fail("unsupported ArrowType list of list (tag 25): nested types are out of scope");
+                t = DType::list(e.type, e.nullable, e.name);
+                break;
+            }
+            case 26: case 27: fail("unsupported ArrowType list (tag " + std::to_string(f) + "): nested types are out of scope");
             case 28: case 33: fail(std::string("unsupported ArrowType ") + (f == 28 ? "struct" : "map") + " (tag " + std::to_string(f) + "): nested types are out of scope");
             default: fail("unsupported ArrowType tag " + std::to_string(f) + " (nested / interval types are out of scope)");
         }
@@ -182,7 +202,10 @@ HostArray decode_list_scalar_ipc(const uint8_t* bytes, size_t n) {
     uint32_t nchildren;
     const uint8_t* children = field.vec(5, &nchildren);
     AURON_CHECK(children && nchildren == 1, "list ScalarValue: malformed child field");
-    out.type = fb_field_type(field.vec_table(children, 0));
+    const FbTable elem = field.vec_table(children, 0);
+    out.type = fb_field_type(elem);
+    out.elem_name = elem.str(0);
+    out.elem_nullable = elem.scalar<uint8_t>(1, 0) != 0;
     AURON_CHECK(next_ipc_message(p, end, &meta, &meta_len, &body, &body_len), "list ScalarValue: missing record batch");
     msg = FbTable::root(meta, meta_len);
     AURON_CHECK(msg.scalar<uint8_t>(1, 0) == 3, "list ScalarValue: second IPC message is not a RecordBatch");
@@ -193,6 +216,10 @@ HostArray decode_list_scalar_ipc(const uint8_t* bytes, size_t n) {
     const uint8_t* bufs = rb.vec(2, &nbufs, 16);     // Buffer{offset, length}
     AURON_CHECK(rb.field_off(3) == 0, "list ScalarValue: compressed IPC bodies are not supported");
     AURON_CHECK(nnodes == 2 && rb.scalar<int64_t>(0, 0) == 1, "list ScalarValue: expected one list row");
+    if (FbTable::rd<int64_t>(nodes + 8) > 0) {   // the list row is NULL: no elements
+        out.list_is_null = true;
+        return out;
+    }
     auto buf = [&](uint32_t i, int64_t* len) -> const uint8_t* {
         AURON_CHECK(i < nbufs, "list ScalarValue: missing buffer");
         int64_t off = FbTable::rd<int64_t>(bufs + 16 * i);
@@ -245,6 +272,22 @@ HostArray decode_list_scalar_ipc(const uint8_t* bytes, size_t n) {
         out.data.assign(cd + (size_t)first * w, cd + (size_t)last * w);
     }
     return out;
+}
+
+bool is_list_scalar_ipc(const uint8_t* bytes, size_t n) {
+    const uint8_t* p = bytes;
+    const uint8_t *meta, *body;
+    uint32_t meta_len;
+    int64_t body_len;
+    if (!next_ipc_message(p, bytes + n, &meta, &meta_len, &body, &body_len)) return false;
+    FbTable msg = FbTable::root(meta, meta_len);
+    if (msg.scalar<uint8_t>(1, 0) != 1) return false;
+    FbTable schema = msg.table(2);
+    if (!schema.ok()) return false;
+    uint32_t nfields;
+    const uint8_t* fields = schema.vec(1, &nfields);
+    if (nfields != 1) return false;
+    return schema.vec_table(fields, 0).scalar<uint8_t>(2, 0) == 12;
 }
 
 ColumnPtr host_array_to_device(Ctx& ctx, const HostArray& a) {
@@ -447,7 +490,14 @@ ExprPtr decode_expr(const uint8_t* b, size_t n) {
                         const uint8_t* ib;
                         size_t in;
                         s.bytes_view(&ib, &in);
-                        e->lit = decode_scalar_ipc(ib, in);
+                        if (is_list_scalar_ipc(ib, in)) {   // a list literal: one list row, broadcast (operators.cc ListExpr)
+                            auto h = std::make_shared<HostArray>(decode_list_scalar_ipc(ib, in));
+                            e->lit.type = DType::list(h->type, h->elem_nullable, h->elem_name.empty() ? "item" : h->elem_name);
+                            e->lit.is_null = h->list_is_null;
+                            e->list_lit = h;
+                        } else {
+                            e->lit = decode_scalar_ipc(ib, in);
+                        }
                     } else s.skip(sw);
                 }
                 break;
@@ -678,6 +728,22 @@ SortExprSpec decode_sort_expr(const uint8_t* b, size_t n) {
     return out;
 }
 
+// list columns pass only through Filter, Project, Limit, Union, Rename, the pass-through nodes, Generate and the Arrow export; the
+// operators that sort, hash, serialise or aggregate rows reject a list column they carry or reference when the plan is built
+static void reject_list_columns(const char* op, const Schema& s) {
+    for (auto& f : s.fields)
+        if (f.type.id == T_LIST) fail(std::string(op) + ": list column " + f.name + " (" + f.type.str() + ") is not supported by this operator");
+}
+static void reject_list_refs(const char* op, const Expr& e, const Schema& s) {
+    if (e.kind == E_COLUMN) {
+        const int i = e.index >= 0 ? e.index : s.index_of(e.name);
+        if (i >= 0 && i < (int)s.fields.size() && s.fields[(size_t)i].type.id == T_LIST)
+            fail(std::string(op) + ": list column " + s.fields[(size_t)i].name + " (" + s.fields[(size_t)i].type.str() + ") is not supported by this operator");
+    }
+    for (auto& c : e.children)
+        if (c) reject_list_refs(op, *c, s);
+}
+
 static OperatorPtr decode_agg(Task& t, const uint8_t* b, size_t n) {
     PbReader r(b, n);
     uint32_t f, w;
@@ -732,6 +798,9 @@ static OperatorPtr decode_agg(Task& t, const uint8_t* b, size_t n) {
         else r.skip(w);
     }
     AURON_CHECK(input, "AggExecNode without input");
+    for (auto& g : groups) reject_list_refs("AggExec", *g, input->out_schema);
+    for (auto& a : aggs)
+        for (auto& c : a.children) reject_list_refs("AggExec", *c, input->out_schema);
     for (size_t i = 0; i < aggs.size(); i++) {
         aggs[i].mode = i < modes.size() ? modes[i] : MODE_PARTIAL;
         aggs[i].name = i < anames.size() ? anames[i] : "";
@@ -776,6 +845,11 @@ static OperatorPtr decode_join(Task& t, const uint8_t* b, size_t n, int kind /*0
         else r.skip(w);
     }
     AURON_CHECK(left && right, "join without both inputs");
+    const char* jname = kind == 1 ? "SortMergeJoinExec" : kind == 2 ? "BroadcastJoinExec" : "HashJoinExec";
+    reject_list_columns(jname, left->out_schema);
+    reject_list_columns(jname, right->out_schema);
+    reject_list_exprs(lk, left->out_schema, "a join key");
+    reject_list_exprs(rk, right->out_schema, "a join key");
     if (kind == 1) return OperatorPtr(new SortMergeJoinExec(std::move(left), std::move(right), lk, rk, sort_opts, jt, schema));
     auto* j = new HashJoinExec(std::move(left), std::move(right), lk, rk, jt, side, schema);
     j->null_aware_anti = null_aware;
@@ -861,6 +935,8 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     } else s.skip(sw);
                 }
                 AURON_CHECK(input, "SortExecNode without input");
+                reject_list_columns("SortExec", input->out_schema);
+                for (auto& k : keys) reject_list_exprs({k.expr}, input->out_schema, "a sort key");
                 out.reset(new SortExec(std::move(input), keys, limit, offset));
                 break;
             }
@@ -896,6 +972,7 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     else if (sf == 3 && sw == 2) id = s.bytes();
                     else s.skip(sw);
                 }
+                reject_list_columns("IpcReaderExec", schema);
                 out = make_ipc_reader(t, schema, id);
                 break;
             }
@@ -976,6 +1053,8 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     } else s.skip(sw);
                 }
                 AURON_CHECK(input, "ExpandExecNode without input");
+                reject_list_columns("ExpandExec", input->out_schema);
+                reject_list_columns("ExpandExec", schema);
                 std::vector<std::vector<ExprPtr>> projs;
                 for (auto& pr : raw) {
                     projs.emplace_back();
@@ -1011,6 +1090,7 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     else s.skip(sw);
                 }
                 AURON_CHECK(input, "WindowExecNode without input");
+                reject_list_columns("WindowExec", input->out_schema);
                 std::vector<ExprPtr> part, order;
                 for (auto& e : raw_part) part.push_back(decode_expr(e.data(), e.size()));
                 for (auto& e : raw_order) order.push_back(decode_sort_expr(e.data(), e.size()).expr);   // (the direction is the sort's business: only equality of neighbours matters here)
@@ -1042,6 +1122,7 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     try {
                         if (field_b) spec.field = decode_field(field_b, field_n);
                         if (type_b) spec.field.type = decode_arrow_type(type_b, type_n);   // return_type repeats the field's type
+                        if (spec.field.type.id == T_LIST) fail("a list result (" + spec.field.type.str() + ") is not supported");
                         for (auto& a : arg_b) spec.args.push_back(decode_expr(a.first, a.second));
                     } catch (const Error& e) {
                         static const char* wfn[] = {"ROW_NUMBER", "RANK", "DENSE_RANK", "LEAD", "NTH_VALUE", "NTH_VALUE_IGNORE_NULLS", "PERCENT_RANK", "CUME_DIST"};
@@ -1052,6 +1133,9 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     }
                     funcs.push_back(std::move(spec));
                 }
+                reject_list_exprs(part, input->out_schema, "a window partition key");
+                reject_list_exprs(order, input->out_schema, "a window order key");
+                for (auto& fs : funcs) reject_list_exprs(fs.args, input->out_schema, "a window function argument");
                 out.reset(new WindowExec(std::move(input), std::move(part), std::move(order), std::move(funcs), limit, out_cols));
                 break;
             }
@@ -1064,10 +1148,61 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     else s.skip(sw);
                 }
                 AURON_CHECK(input, "IpcWriterExecNode without input");
+                reject_list_columns("IpcWriterExec", input->out_schema);
                 out = make_ipc_writer(t, std::move(input), rid);
                 break;
             }
-            case 5: out = make_parquet_scan(t, sb, sn); break;
+            case 5:
+                out = make_parquet_scan(t, sb, sn);
+                reject_list_columns("ParquetScanExec", out->out_schema);   // Parquet LIST columns are not read
+                break;
+            case 23: {   // GenerateExecNode{input=1, generator=2{func=1, udtf=2, child=3}, required_child_output=3, generator_output=4, outer=5}
+                OperatorPtr input;
+                bool has_gen = false, outer = false, has_udtf = false;
+                int func = 0;
+                std::vector<std::vector<uint8_t>> raw_child;   // resolved against the input's schema: decoded after it
+                std::vector<std::string> req;
+                std::vector<Field> gout;
+                while (s.next(&sf, &sw)) {
+                    if (sf == 1 && sw == 2) input = plan_field(t, s);
+                    else if (sf == 2 && sw == 2) {
+                        has_gen = true;
+                        const uint8_t* gb;
+                        size_t gn;
+                        s.bytes_view(&gb, &gn);
+                        PbReader g(gb, gn);
+                        uint32_t gf, gw;
+                        while (g.next(&gf, &gw)) {
+                            if (gf == 1 && gw == 0) func = (int)g.varint();
+                            else if (gf == 2 && gw == 2) {
+                                has_udtf = true;
+                                g.skip(gw);
+                            } else if (gf == 3 && gw == 2) {
+                                const uint8_t* cb;
+                                size_t cn;
+                                g.bytes_view(&cb, &cn);
+                                raw_child.emplace_back(cb, cb + cn);
+                            } else g.skip(gw);
+                        }
+                    } else if (sf == 3 && sw == 2) req.push_back(s.bytes());
+                    else if (sf == 4 && sw == 2) {
+                        const uint8_t* fb;
+                        size_t fn;
+                        s.bytes_view(&fb, &fn);
+                        gout.push_back(decode_field(fb, fn));
+                    } else if (sf == 5 && sw == 0) outer = s.varint() != 0;
+                    else s.skip(sw);
+                }
+                AURON_CHECK(input, "GenerateExecNode without input");
+                if (!has_gen) fail("GenerateExec without a generator is not native in auron_b200");
+                if (func == 2) fail("generate function JsonTuple is not native in auron_b200");
+                if (func == 10000 || has_udtf) fail("generate function Udtf is not native in auron_b200");
+                if (func != GEN_EXPLODE && func != GEN_POS_EXPLODE) fail("generate function #" + std::to_string(func) + " is not native in auron_b200");
+                if (raw_child.size() != 1) fail(std::string(func == GEN_POS_EXPLODE ? "PosExplode" : "Explode") + " takes one child expression, got " + std::to_string(raw_child.size()));
+                ExprPtr child = decode_expr_required(raw_child[0].data(), raw_child[0].size());
+                out.reset(new GenerateExec(std::move(input), func, child, std::move(req), std::move(gout), outer));
+                break;
+            }
             case 2: {   // ShuffleWriterExecNode{input=1, ...}
                 OperatorPtr input;
                 PbReader s2(sb, sn);
@@ -1076,6 +1211,7 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                     else s2.skip(sw);
                 }
                 AURON_CHECK(input, "ShuffleWriterExecNode without input");
+                reject_list_columns("ShuffleWriterExec", input->out_schema);
                 out = make_shuffle_writer(t, std::move(input), sb, sn);
                 break;
             }

@@ -528,6 +528,8 @@ OperatorPtr make_ipc_writer(Task& t, OperatorPtr input, const std::string& consu
     op->ipc_consumer_id = consumer_id;
     op->zstd = t.conf("SPARK_IO_COMPRESSION_CODEC", "AURON_IO_COMPRESSION_CODEC", "lz4") == "zstd";
     op->zstd_level = atoi(t.conf("SPARK_IO_COMPRESSION_ZSTD_LEVEL", "AURON_IO_COMPRESSION_ZSTD_LEVEL", "1").c_str());
+    reject_list_exprs(op->hash_exprs, input->out_schema, "a shuffle partitioning key");
+    for (auto& k : op->range_keys) reject_list_exprs({k.expr}, input->out_schema, "a shuffle partitioning key");
     op->children.push_back(std::move(input));
     return op;
 }
@@ -614,6 +616,8 @@ OperatorPtr make_shuffle_writer(Task& t, OperatorPtr input, const uint8_t* node,
     // spark.io.compression.codec (lz4 | zstd) and spark.io.compression.zstd.level (conf.rs:46-47, ipc_compression.rs:180-200)
     op->zstd = t.conf("SPARK_IO_COMPRESSION_CODEC", "AURON_IO_COMPRESSION_CODEC", "lz4") == "zstd";
     op->zstd_level = atoi(t.conf("SPARK_IO_COMPRESSION_ZSTD_LEVEL", "AURON_IO_COMPRESSION_ZSTD_LEVEL", "1").c_str());
+    reject_list_exprs(op->hash_exprs, input->out_schema, "a shuffle partitioning key");
+    for (auto& k : op->range_keys) reject_list_exprs({k.expr}, input->out_schema, "a shuffle partitioning key");
     op->children.push_back(std::move(input));
     return op;
 }

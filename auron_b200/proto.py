@@ -75,6 +75,8 @@ def arrow_type(t: pa.DataType) -> bytes:
         return f_bytes(20, body)
     if pa.types.is_decimal128(t):
         return f_bytes(24, f_varint(1, t.precision) + f_varint(2, t.scale))
+    if pa.types.is_list(t):
+        return f_bytes(25, f_bytes(1, field(t.value_field.name, t.value_type, t.value_field.nullable)))   # List{field_type}
     raise NotImplementedError(str(t))
 
 
@@ -322,6 +324,19 @@ def window(inp: bytes, window_exprs: list[bytes], partition_spec: list[bytes], o
     if group_limit is not None:
         body += f_bytes(5, f_varint(1, group_limit, always=True))
     return f_bytes(22, body + f_varint(6, int(output_window_cols)))
+
+
+GENERATE_FUNCTION = {"Explode": 0, "PosExplode": 1, "JsonTuple": 2, "Udtf": 10000}
+
+
+def generate(inp: bytes, func: str, child: bytes, required_child_output: list[str], generator_output: list[tuple[str, pa.DataType, bool]],
+             outer: bool = False) -> bytes:
+    """PhysicalPlanNode{generate{input, generator{func, child}, required_child_output, generator_output, outer}} (auron.proto:593-612;
+    NativeGenerateBase.scala); generator_output holds (name, type, nullable) per generated column"""
+    gen = f_varint(1, GENERATE_FUNCTION[func]) + f_bytes(3, child)
+    body = f_bytes(1, inp) + f_bytes(2, gen) + b"".join(f_str(3, n) for n in required_child_output)
+    body += b"".join(f_bytes(4, field(n, t, nl)) for n, t, nl in generator_output)
+    return f_bytes(23, body + f_varint(5, int(outer)))
 
 
 def ipc_writer(inp: bytes, consumer_resource_id: str) -> bytes:

@@ -2,7 +2,7 @@
 time per launch site from the library's CUDA-event timers (AURON_PROFILE=1).  These are the operator-level numbers the
 north star asks for next to the config-2 bench line; they are not bench.py lines.
 
-    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [scalar] [casts] [window]
+    python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [scalar] [casts] [window] [generate]
 
   join     cfg 3: store_sales (N rows: ss_sold_date_sk int32, ss_item_sk int32, ss_quantity int32) JOIN date_dim (73,049 rows:
            d_date_sk int32, d_year int32) on the date key, inner, build = date_dim
@@ -26,6 +26,9 @@ north star asks for next to the config-2 bench line; they are not bench.py lines
   window   WindowExec over N pre-sorted rows (p int32, ~1,000 rows per partition; o int64; v decimal(17,2), 5 % NULL; s utf8 8-24 B)
            in device batches of 16M rows, so the running state carries across batch edges: ROW_NUMBER, RANK, SUM(v), AVG(v), MAX(s),
            COUNT(v) partitioned by p ordered by o, + COUNT / SUM so that one row leaves the GPU
+  generate LATERAL VIEW explode(split(s, ',')) + COUNT grouped by the element over N rows of 34 B strings (five 6-letter words from a
+           vocabulary of 1,000, four separators), in device batches of 16M rows.  Reports the device time of the split kernels and of
+           the generate gather with their algorithmic bytes, then the Filter -> Project leg, so that both come from the same run
 """
 import os
 import sys
@@ -400,3 +403,38 @@ if "window" in which:
     run(plan, f"window ROW_NUMBER, RANK, SUM(dec), AVG(dec), MAX(utf8), COUNT over {N} rows in {(N + CHUNK - 1) // CHUNK} batches", N, steps=3,
         alg={"window_scan": scan_b, "take": 2 * (s_bytes + 4 * N)})
     runtime.drop_device_resource("win")
+
+if "generate" in which:
+    import subprocess
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"== generate leg on: {gpu}")
+    U = pa.string()
+    vocab = rng.integers(97, 123, (1000, 6), dtype=np.uint8)
+    W, K = 6, 5   # word length, words per row: rows of K * W + K - 1 = 34 bytes
+    row_b = K * W + K - 1
+    for start in range(0, N, CHUNK):
+        n = min(CHUNK, N - start)
+        mat = np.full((n, row_b), ord(","), dtype=np.uint8)
+        ids = rng.integers(0, 1000, (n, K))
+        for k in range(K):
+            mat[:, k * (W + 1):k * (W + 1) + W] = vocab[ids[:, k]]
+        offs = np.arange(0, (n + 1) * row_b, row_b, dtype=np.int32)
+        s_arr = pa.Array.from_buffers(U, n, [None, pa.py_buffer(offs), pa.py_buffer(mat.reshape(-1))])
+        runtime.put_device_batch("gen", pa.record_batch([s_arr], names=["s"]))
+    LU = pa.list_(U)
+    proj = P.projection(P.ffi_reader(pa.schema([("s", U)]), "gen"), [P.scalar_fn("Spark_StringSplit", [P.col("s"), P.lit(",", U)], LU)], ["p"], [LU])
+    gen = P.generate(proj, "Explode", P.col("p"), [], [("w", U, True)])
+    plan = P.agg(gen, [P.col("w")], ["w"], [P.agg_expr("COUNT", [P.col("w")], pa.int64())], ["c"], ["PARTIAL"])
+    with runtime.Task(P.task_definition(plan)) as task:   # every word once per row and position: the counts add up to K * N
+        total = sum(sum(b.column(1).to_pylist()) for b in task)
+    assert total == K * N, total
+    # algorithmic bytes, inputs once + outputs once: split reads the strings and their offsets and writes the pieces (the bytes less the
+    # separators), their offsets and the list offsets; the gather reads and writes the pieces with their offsets
+    piece_b, pieces = K * W * N, K * N
+    split_b = (row_b + 4) * N + piece_b + 4 * pieces + 4 * N
+    take_b = 2 * (piece_b + 4 * pieces)
+    run(plan, f"explode(split(s, ',')) -> COUNT by element over {N} rows of {row_b} B", N, steps=4,
+        alg={"string_split": split_b, "take": take_b})
+    runtime.drop_device_resource("gen")
+    filter_project_leg()
