@@ -63,7 +63,33 @@ std::string describe(const char* path) {
           << ",\"has_logical_type\":" << (e.has_logical_type ? "true" : "false") << ",\"logical\":" << e.logical << ",\"ts_unit\":" << e.ts_unit
           << ",\"ts_utc\":" << (e.ts_utc ? "true" : "false") << ",\"int_bits\":" << e.int_bits << ",\"int_signed\":" << (e.int_signed ? "true" : "false") << "}";
     }
-    o << "],\"row_groups\":[";
+    // the schema as a tree: every leaf with its levels and the top-level field it belongs to (a schema that is not a tree is
+    // described without it, as far as the flat walk goes)
+    pq::SchemaTree tree;
+    std::string tree_error;
+    try {
+        tree = pq::walk_schema(md);
+    } catch (const std::exception& e) {
+        tree_error = e.what();
+        tree = pq::SchemaTree();
+    }
+    o << "],\"leaves\":[";
+    for (size_t i = 0; i < tree.leaves.size(); i++) {
+        const auto& l = tree.leaves[i];
+        const auto& f = tree.fields[(size_t)l.field];
+        o << (i ? "," : "") << "{\"path\":" << quote(l.path) << ",\"chunk\":" << l.chunk << ",\"element\":" << l.element << ",\"max_def\":" << l.max_def
+          << ",\"max_rep\":" << l.max_rep << ",\"field\":" << quote(f.name) << ",\"shape\":" << quote(pq::shape_name(f.shape)) << ",\"read\":"
+          << (f.leaf == (int32_t)i ? "true" : "false") << "}";
+    }
+    o << "],\"fields\":[";
+    for (size_t i = 0; i < tree.fields.size(); i++) {
+        const auto& f = tree.fields[i];
+        o << (i ? "," : "") << "{\"name\":" << quote(f.name) << ",\"shape\":" << quote(pq::shape_name(f.shape)) << ",\"leaf\":" << f.leaf
+          << ",\"list_def\":" << f.list_def << ",\"elem_def\":" << f.elem_def << "}";
+    }
+    o << "]";
+    if (!tree_error.empty()) o << ",\"schema_error\":" << quote(tree_error);
+    o << ",\"row_groups\":[";
     for (size_t g = 0; g < md.row_groups.size(); g++) {
         const auto& rg = md.row_groups[g];
         o << (g ? "," : "") << "{\"num_rows\":" << rg.num_rows << ",\"total_byte_size\":" << rg.total_byte_size << ",\"columns\":[";
@@ -86,7 +112,10 @@ std::string describe(const char* path) {
             // the integers, count + byte total + FNV-1a of the PLAIN transcription of the strings)
             int64_t split_pages = 0, split_head_out = 0, split_stored = 0, delta_pages = 0, delta_values = 0, delta_bytes = 0;
             uint64_t delta_sum = 0, delta_fnv = 1469598103934665603ull;
-            const int max_def = (c + 1 < md.schema.size() && md.schema[c + 1].repetition == 1) ? 1 : 0;   // flat schemas: leaf c is element c + 1
+            // levels of the chunk's leaf (a schema that is not a tree: element c + 1, as for a flat schema)
+            const int max_def = c < tree.leaves.size() ? tree.leaves[c].max_def : (c + 1 < md.schema.size() && md.schema[c + 1].repetition == 1) ? 1 : 0;
+            const int max_rep = c < tree.leaves.size() ? tree.leaves[c].max_rep : 0;
+            int64_t level_pages = 0, level_rows = 0, level_values = 0;
             std::string encodings;
             while (pos < cm.total_compressed) {
                 pq::PageHeader h = pq::parse_page_header(chunk.data() + pos, (size_t)(cm.total_compressed - pos));
@@ -128,15 +157,40 @@ std::string describe(const char* path) {
                     have_body = true;
                 }
                 const size_t blen = have_body ? out.size() - 8 : 0;   // bytes of `out` that belong to the page (sizes in a damaged header are not trusted)
+                // leaves under a repeated field: rows (rep == 0) and non-null values (def == max_def) of the page, counted from its levels with
+                // the walk the scan uses for v1 list pages
+                if (max_rep > 0 && (h.type == pq::PAGE_DATA || h.type == pq::PAGE_DATA_V2)) {
+                    const uint8_t *rp = nullptr, *dp = nullptr;
+                    size_t rl = 0, dl = 0;
+                    if (h.type == pq::PAGE_DATA_V2) {
+                        AURON_CHECK(h.rep_bytes >= 0 && h.def_bytes >= 0 && (int64_t)h.rep_bytes + h.def_bytes <= h.compressed_size, "corrupt parquet page levels");
+                        rp = body, rl = (size_t)h.rep_bytes, dp = body + h.rep_bytes, dl = (size_t)h.def_bytes;
+                    } else if (have_body) {
+                        uint32_t a = 0, b = 0;
+                        AURON_CHECK(blen >= 4, "corrupt parquet page");
+                        memcpy(&a, out.data(), 4);
+                        AURON_CHECK((size_t)a + 8 <= blen, "corrupt parquet page levels");
+                        memcpy(&b, out.data() + 4 + a, 4);
+                        AURON_CHECK((size_t)a + 8 + b <= blen, "corrupt parquet page levels");
+                        rp = out.data() + 4, rl = a, dp = out.data() + 8 + a, dl = b;
+                    }
+                    if (rp) {
+                        auto bw = [](int m) { int b = 0; while ((1 << b) <= m) b++; return b; };
+                        level_rows += pq::hybrid_count(rp, rl, bw(max_rep), h.num_values, 0);
+                        level_values += pq::hybrid_count(dp, dl, bw(max_def), h.num_values, (uint32_t)max_def);
+                        level_pages++;
+                    }
+                }
                 const bool delta = h.encoding == pq::ENC_DELTA_BINARY_PACKED || h.encoding == pq::ENC_DELTA_LENGTH_BYTE_ARRAY || h.encoding == pq::ENC_DELTA_BYTE_ARRAY;
                 if (have_body && delta && (h.type == pq::PAGE_DATA || h.type == pq::PAGE_DATA_V2)) {
                     size_t vo = 0;   // value section inside `out`
-                    if (h.type == pq::PAGE_DATA && max_def > 0) {
-                        AURON_CHECK(blen >= 4, "corrupt parquet page");
-                        uint32_t dl = 0;
-                        memcpy(&dl, out.data(), 4);
-                        vo = 4 + (size_t)dl;
-                    }
+                    if (h.type == pq::PAGE_DATA)   // [u32 length][repetition levels] if max_rep > 0, [u32 length][definition levels] if max_def > 0
+                        for (int sec = (max_rep > 0 ? 0 : 1); sec < (max_def > 0 ? 2 : 1); sec++) {
+                            AURON_CHECK(vo + 4 <= blen, "corrupt parquet page");
+                            uint32_t dl = 0;
+                            memcpy(&dl, out.data() + vo, 4);
+                            vo += 4 + (size_t)dl;
+                        }
                     AURON_CHECK(vo <= blen && h.num_values >= 0, "corrupt parquet page levels");
                     const size_t vlen = blen - vo;
                     if (h.encoding == pq::ENC_DELTA_BINARY_PACKED) {
@@ -168,7 +222,9 @@ std::string describe(const char* path) {
             o << ",\"data_pages\":" << pages << ",\"dictionary_pages\":" << dict_pages << ",\"page_values\":" << values << ",\"pages_uncompressed\":" << unc
               << ",\"snappy_pages_decompressed\":" << snappy_checked << ",\"snappy_split_pages\":" << split_pages << ",\"snappy_split_head_bytes\":" << split_head_out
               << ",\"snappy_split_stored_bytes\":" << split_stored << ",\"delta_pages\":" << delta_pages << ",\"delta_values\":" << delta_values << ",\"delta_sum\":\""
-              << delta_sum << "\",\"delta_string_bytes\":" << delta_bytes << ",\"delta_fnv\":\"" << delta_fnv << "\",\"page_encodings\":[" << encodings << "]}";
+              << delta_sum << "\",\"delta_string_bytes\":" << delta_bytes << ",\"delta_fnv\":\"" << delta_fnv << "\",\"page_encodings\":[" << encodings << "]";
+            if (max_rep > 0) o << ",\"level_pages\":" << level_pages << ",\"level_rows\":" << level_rows << ",\"level_values\":" << level_values;
+            o << "}";
         }
         o << "]}";
     }

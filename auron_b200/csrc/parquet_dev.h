@@ -85,6 +85,30 @@ void pq_fix_v1_pages(Ctx& ctx, PqPage* pages, int n, const PqDecompResult* resul
 // status (int32, may be the decompression status word) is set to 0x40000000 + page when a stream is malformed
 void pq_delta_to_plain(Ctx& ctx, PqPage* pages, int n, uint8_t* scratch, int width, int32_t* status);
 
+// ---- one-level LIST columns (k_parquet_levels.cu).  The element values of a list page are contiguous and decode with the page
+// decoders above as a required column; the level streams of the pages give the list layout.
+struct PqLevelPage {
+    const uint8_t* rep;       // repetition levels (hybrid RLE / bit-packed)
+    const uint8_t* def;       // definition levels
+    int32_t rep_len, def_len;
+    int32_t n_slots;          // level slots of the page (its num_values: elements, empty lists and NULL lists)
+    int32_t slot_start;       // first slot of the page within the batch's column
+};
+struct PqListShape {
+    int32_t rep_bw, def_bw;   // bit widths of max_rep (1) and max_def
+    int32_t list_def;         // def < list_def: a NULL list (0: the list is required)
+    int32_t elem_def;         // list_def <= def < elem_def: an empty list; def >= elem_def: an element
+    int32_t max_def;          // an element is NULL unless def == max_def
+};
+// Level pass over the n_slots slots of a batch's list column: offsets[0, n_rows] (row r owns elements [offsets[r], offsets[r + 1])),
+// validity (n_rows bits, zeroed by the caller; nullptr when list_def == 0) and elem_idx[e] = index of element e's value among the
+// non-null values, -1 for a NULL element.  counts (device, int64[4]): rows found, elements, non-null values, status (0 = ok, else
+// 1 + a page whose levels are malformed).  Rows past n_rows are counted, never written.
+void pq_list_levels(Ctx& ctx, const PqLevelPage* pages, int n_pages, int64_t n_slots, int64_t n_rows, const PqListShape& s, int32_t* offsets,
+                    uint32_t* validity, int32_t* elem_idx, int64_t* counts);
+// idx[e] = idx[e] < 0 ? -1 : value_idx[idx[e]] for e < n, in place (a list of strings: element -> value-table entry, one byte gather)
+void pq_compose_index(Ctx& ctx, int32_t* idx, const int32_t* value_idx, int64_t n);
+
 // scout + decode of one column; or in three steps, so that one scout launch serves every column of a batch
 void pq_decode_pages(Ctx& ctx, const PqColumnArgs& a, const std::vector<PqPage>& host_pages);
 struct PqPrepared {

@@ -2,6 +2,7 @@
 // Snappy block decompressor (host side of ParquetScanExec).
 #include "parquet_meta.h"
 
+#include <algorithm>
 #include <cstring>
 
 namespace auron {
@@ -122,6 +123,8 @@ void read_logical_type(TReader& r, SchemaElement& e) {
         int t2;
         switch (id) {
             case 1: e.logical = LK_STRING; r.skip(t); break;
+            case 2: e.map_annot = true; r.skip(t); break;
+            case 3: e.list_annot = true; r.skip(t); break;
             case 6: e.logical = LK_DATE; r.skip(t); break;
             case 5:
                 e.logical = LK_DECIMAL;
@@ -201,6 +204,8 @@ SchemaElement read_schema_element(TReader& r) {
         }
     }
     if (!e.has_logical_type) logical_from_converted(e);
+    if (e.converted_type == 3) e.list_annot = true;   // LIST
+    if (e.converted_type == 1 || e.converted_type == 2) e.map_annot = true;   // MAP, MAP_KEY_VALUE
     return e;
 }
 Statistics read_statistics(TReader& r) {
@@ -322,6 +327,99 @@ FileMeta parse_file_meta(const uint8_t* buf, size_t len) {
             if (s.legacy_max) s.has_max = s.legacy_max = false, s.max_value.clear();
         }
     return m;
+}
+
+const char* shape_name(int shape) {
+    switch (shape) {
+        case SHAPE_FLAT: return "primitive";
+        case SHAPE_LIST: return "list";
+        case SHAPE_STRUCT: return "struct";
+        case SHAPE_MAP: return "map";
+        case SHAPE_LIST_OF_LIST: return "list of lists";
+        case SHAPE_LIST_OF_STRUCT: return "list of structs";
+        case SHAPE_LIST_OF_MAP: return "list of maps";
+        default: return "malformed list";
+    }
+}
+
+namespace {
+// pre-order walk of element i's subtree; returns the index behind it.  def / rep: levels of the parent.
+size_t walk_node(const std::vector<SchemaElement>& s, size_t i, int field, const std::string& parent, int def, int rep, int depth, SchemaTree& t,
+                 std::vector<std::vector<size_t>>& kids) {
+    AURON_CHECK(i < s.size(), "parquet: the schema ends inside a group");
+    AURON_CHECK(depth <= 64, "parquet: schema nested too deeply");
+    const SchemaElement& e = s[i];
+    AURON_CHECK(e.num_children >= 0 && (size_t)e.num_children < s.size(), "parquet: bad num_children in the schema");
+    const std::string path = parent.empty() ? e.name : parent + "." + e.name;
+    def += e.repetition != 0;   // OPTIONAL or REPEATED
+    rep += e.repetition == 2;
+    if (e.num_children == 0) {
+        t.leaves.push_back(SchemaLeaf{(int32_t)t.leaves.size(), (int32_t)i, field, def, rep, path});
+        return i + 1;
+    }
+    size_t j = i + 1;
+    for (int c = 0; c < e.num_children; c++) {
+        kids[i].push_back(j);
+        j = walk_node(s, j, field, path, def, rep, depth + 1, t, kids);
+    }
+    return j;
+}
+}  // namespace
+
+SchemaTree walk_schema(const FileMeta& m) {
+    SchemaTree t;
+    const auto& s = m.schema;
+    AURON_CHECK(!s.empty(), "empty parquet schema");
+    std::vector<std::vector<size_t>> kids(s.size());
+    size_t j = 1;
+    for (int c = 0; c < s[0].num_children; c++) {
+        TopField f;
+        f.element = (int32_t)j;
+        AURON_CHECK(j < s.size(), "parquet: the schema ends inside the root");
+        f.name = s[j].name;
+        const int32_t first_leaf = (int32_t)t.leaves.size();
+        j = walk_node(s, j, (int)t.fields.size(), "", 0, 0, 0, t, kids);
+        const SchemaElement& e = s[(size_t)f.element];
+        const int opt = e.repetition == 1 ? 1 : 0;
+        auto list_of_leaf = [&] {
+            f.shape = SHAPE_LIST;
+            f.leaf = first_leaf;
+            f.list_def = e.repetition == 2 ? 0 : opt;   // (a bare repeated field is a required list)
+            f.elem_def = f.list_def + 1;
+        };
+        if (e.num_children == 0) {
+            if (e.repetition == 2) list_of_leaf();   // a repeated primitive outside any LIST group: list<required element>
+            else {
+                f.shape = SHAPE_FLAT;
+                f.leaf = first_leaf;
+            }
+        } else if (e.map_annot) {
+            f.shape = SHAPE_MAP;
+        } else if (e.repetition == 2) {
+            f.shape = SHAPE_LIST_OF_STRUCT;   // a repeated group outside any LIST group: list<required struct>
+        } else if (!e.list_annot) {
+            f.shape = SHAPE_STRUCT;
+        } else if (kids[(size_t)f.element].size() == 1 && s[kids[(size_t)f.element][0]].repetition == 2) {
+            const size_t r = kids[(size_t)f.element][0];
+            const SchemaElement& R = s[r];
+            if (R.num_children == 0) list_of_leaf();   // 2-level: the repeated primitive is the element
+            else if (R.num_children > 1 || R.name == "array" || R.name == e.name + "_tuple") f.shape = SHAPE_LIST_OF_STRUCT;   // the repeated group is the element
+            else {   // 3-level: the repeated group's only field is the element, whatever the names
+                const SchemaElement& E = s[kids[r][0]];
+                if (E.num_children == 0) {
+                    if (E.repetition == 2) f.shape = SHAPE_LIST_OF_LIST;
+                    else list_of_leaf();
+                } else if (E.list_annot || E.repetition == 2) f.shape = SHAPE_LIST_OF_LIST;
+                else if (E.map_annot) f.shape = SHAPE_LIST_OF_MAP;
+                else f.shape = SHAPE_LIST_OF_STRUCT;
+            }
+        } else {
+            f.shape = SHAPE_OTHER;   // a LIST group must hold exactly one repeated field
+        }
+        t.fields.push_back(f);
+    }
+    AURON_CHECK(j == s.size(), "parquet: schema elements outside the root's tree");
+    return t;
 }
 
 PageHeader parse_page_header(const uint8_t* buf, size_t len) {
@@ -489,6 +587,42 @@ bool snappy_split(const uint8_t* p, int64_t n, int64_t unc, int max_tokens, int6
         }
     }
     return out == unc;
+}
+static bool delta_varint(const uint8_t* p, size_t n, size_t& pos, uint64_t& v);
+int64_t hybrid_count(const uint8_t* p, size_t n, int bw, int64_t num, uint32_t match) {
+    AURON_CHECK(bw >= 0 && bw <= 8, "parquet: level bit width out of range");
+    size_t pos = 0;
+    int64_t seen = 0, hits = 0;
+    while (seen < num) {
+        uint64_t h = 0;
+        AURON_CHECK(delta_varint(p, n, pos, h), "parquet: level stream ends early");
+        if (h & 1) {   // bit-packed: (h >> 1) groups of 8 values
+            const uint64_t groups = h >> 1;
+            AURON_CHECK(groups <= (n - pos) && groups * (uint64_t)bw <= n - pos, "parquet: level stream ends early");
+            const int64_t cnt = (int64_t)std::min<uint64_t>(groups * 8, (uint64_t)(num - seen));
+            for (int64_t i = 0; i < cnt; i++) {
+                uint32_t v = 0;
+                for (int k = 0; k < bw; k++) {
+                    const uint64_t b = (uint64_t)i * bw + k;
+                    v |= (uint32_t)((p[pos + (b >> 3)] >> (b & 7)) & 1) << k;
+                }
+                hits += v == match;
+            }
+            seen += cnt;
+            pos += (size_t)(groups * bw);
+        } else {
+            const uint64_t cnt = h >> 1;
+            const int nb = (bw + 7) / 8;
+            AURON_CHECK(cnt > 0 && pos + nb <= n, "parquet: malformed level run");
+            uint32_t v = 0;
+            for (int k = 0; k < nb; k++) v |= (uint32_t)p[pos + k] << (8 * k);
+            pos += nb;
+            const int64_t take = (int64_t)std::min<uint64_t>(cnt, (uint64_t)(num - seen));
+            hits += v == match ? take : 0;
+            seen += take;
+        }
+    }
+    return hits;
 }
 // ---- DELTA_LENGTH_BYTE_ARRAY / DELTA_BYTE_ARRAY string pages are rewritten as PLAIN on the host (each value of the second
 // depends on the bytes of the one before it; both are rare next to dictionary and PLAIN pages)

@@ -28,6 +28,7 @@ struct SchemaElement {
     bool ts_utc = false;             // LK_TIMESTAMP: isAdjustedToUTC
     int32_t int_bits = 0;            // LK_INTEGER: 8, 16, 32 or 64
     bool int_signed = true;          // LK_INTEGER
+    bool list_annot = false, map_annot = false;   // groups: LIST / MAP (or MAP_KEY_VALUE), from logicalType or converted_type
     // min / max statistics are ordered as signed values (the only order the legacy min / max fields may be read in)
     bool signed_order() const {
         if (logical == LK_INTEGER) return int_signed;
@@ -69,6 +70,34 @@ struct PageHeader {
     int32_t header_len = 0;   // bytes consumed by the header itself
 };
 
+// ---- the schema as a tree (parquet-format LogicalTypes.md, "Nested Types" and its backward-compatibility rules)
+// What the scan makes of one top-level field.  Only FLAT and LIST (a one-level list of a primitive) are read.
+enum FieldShape { SHAPE_FLAT = 0, SHAPE_LIST = 1, SHAPE_STRUCT = 2, SHAPE_MAP = 3, SHAPE_LIST_OF_LIST = 4, SHAPE_LIST_OF_STRUCT = 5, SHAPE_LIST_OF_MAP = 6,
+                  SHAPE_OTHER = 7 };
+const char* shape_name(int shape);
+struct SchemaLeaf {
+    int32_t chunk;        // column-chunk index in every row group (leaves are numbered in schema order)
+    int32_t element;      // index into FileMeta::schema
+    int32_t field;        // index into SchemaTree::fields of the top-level field it belongs to
+    int32_t max_def, max_rep;
+    std::string path;     // dotted path from the root (ColumnMetaData.path_in_schema)
+};
+struct TopField {
+    int32_t element;      // index into FileMeta::schema
+    std::string name;
+    int32_t shape = SHAPE_OTHER;
+    int32_t leaf = -1;    // SHAPE_FLAT: its leaf; SHAPE_LIST: the element's leaf (index into SchemaTree::leaves)
+    // SHAPE_LIST: a level slot with def < list_def is a NULL list, one with def < elem_def an empty list, every other slot holds an
+    // element, NULL unless def == the leaf's max_def
+    int32_t list_def = 0, elem_def = 0;
+};
+struct SchemaTree {
+    std::vector<SchemaLeaf> leaves;
+    std::vector<TopField> fields;
+};
+// throws auron::Error when the element list is not a tree rooted at element 0
+SchemaTree walk_schema(const FileMeta& m);
+
 // throws auron::Error on malformed input
 FileMeta parse_file_meta(const uint8_t* buf, size_t len);
 PageHeader parse_page_header(const uint8_t* buf, size_t len);
@@ -84,6 +113,9 @@ struct LitPiece {
 // [0, *head_in) / [0, *head_out) are the compressed / uncompressed bytes up to and including the last back reference and `pieces` the
 // literals behind it (offsets into p).
 bool snappy_split(const uint8_t* p, int64_t n, int64_t unc, int max_tokens, int64_t* head_in, int64_t* head_out, std::vector<LitPiece>* pieces);
+// How many of the first `num` values of an RLE / bit-packed hybrid stream of bit width `bw` at p[0, n) equal `match` (the rows of a
+// list page: rep == 0; its non-null values: def == max_def).  Throws when the stream ends early.
+int64_t hybrid_count(const uint8_t* p, size_t n, int bw, int64_t num, uint32_t match);
 // one DELTA_BINARY_PACKED stream at p[pos...] -> values; pos ends behind the stream
 // (a stream may not announce more than `max_values` values: the page header's count -- zero-width miniblocks cost no input bytes)
 void delta_binary_decode(const uint8_t* p, size_t n, size_t& pos, std::vector<int64_t>& out, size_t max_values);

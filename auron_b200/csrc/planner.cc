@@ -1153,8 +1153,7 @@ static OperatorPtr decode_plan(Task& t, const uint8_t* b, size_t n) {
                 break;
             }
             case 5:
-                out = make_parquet_scan(t, sb, sn);
-                reject_list_columns("ParquetScanExec", out->out_schema);   // Parquet LIST columns are not read
+                out = make_parquet_scan(t, sb, sn);   // (reads one-level LIST columns of flat elements; rejects list partition columns)
                 break;
             case 23: {   // GenerateExecNode{input=1, generator=2{func=1, udtf=2, child=3}, required_child_output=3, generator_output=4, outer=5}
                 OperatorPtr input;

@@ -118,9 +118,13 @@ struct PqFileSpec {
     int64_t size = 0, range_start = -1, range_end = -1;
     std::vector<Literal> partition_values;   // Hive partition directory values, one per column of the partition schema
 };
-struct LeafColumn {
-    int leaf_index;
-    pq::SchemaElement el;
+struct LeafColumn {            // one top-level field of the file (pq::walk_schema)
+    int leaf_index;            // column chunk of the leaf the scan reads (lists: the element's), -1 = none
+    pq::SchemaElement el;      // that leaf
+    std::string name;          // the top-level field's name
+    std::string path;          // the leaf's dotted path
+    int shape = pq::SHAPE_FLAT;
+    int max_def = 0, max_rep = 0, list_def = 0, elem_def = 0;
 };
 
 struct ParquetScanExec : Operator, FusedScanSource {
@@ -265,12 +269,31 @@ struct ParquetScanExec : Operator, FusedScanSource {
         read_at(t, *fs, size - 8 - flen, footer.data(), flen);
         fs->meta = pq::parse_file_meta(footer.data(), footer.size());
         AURON_CHECK(!fs->meta.schema.empty(), "empty parquet schema");
-        int leaf = 0;
-        for (size_t i = 1; i < fs->meta.schema.size(); i++) {
-            const auto& el = fs->meta.schema[i];
-            AURON_CHECK(el.num_children == 0, "nested parquet columns are out of scope (" + el.name + ")");
-            AURON_CHECK(el.repetition != 2, "repeated parquet columns are out of scope (" + el.name + ")");
-            fs->leaves.push_back({leaf++, el});
+        // every top-level field with its shape; nested fields the query does not read cost nothing here
+        const pq::SchemaTree tree = pq::walk_schema(fs->meta);
+        for (const auto& tf : tree.fields) {
+            LeafColumn lc;
+            lc.leaf_index = -1;
+            lc.el = fs->meta.schema[(size_t)tf.element];
+            lc.name = tf.name;
+            lc.path = tf.name;
+            lc.shape = tf.shape;
+            lc.list_def = tf.list_def;
+            lc.elem_def = tf.elem_def;
+            if (tf.leaf >= 0) {
+                const pq::SchemaLeaf& l = tree.leaves[(size_t)tf.leaf];
+                lc.leaf_index = l.chunk;
+                lc.el = fs->meta.schema[(size_t)l.element];
+                lc.path = l.path;
+                lc.max_def = l.max_def;
+                lc.max_rep = l.max_rep;
+            }
+            fs->leaves.push_back(lc);
+        }
+        for (int pj : projection) {   // a projected field of a shape the scan does not read fails here, with rows or without
+            if (is_part_col(pj) || table_schema.fields[(size_t)pj].type.id == T_NULL) continue;
+            const int li = find_leaf(*fs, table_schema.fields[(size_t)pj].name);
+            if (li >= 0) check_shape(fs->leaves[(size_t)li], table_schema.fields[(size_t)pj]);
         }
         for (size_t g = 0; g < fs->meta.row_groups.size(); g++) {
             const auto& rg = fs->meta.row_groups[g];
@@ -295,7 +318,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
     bool row_group_pruned(const FileState& f, const pq::RowGroup& rg) const {
         for (size_t i = 0; i < prune_cols.size(); i++) {
             const int li = find_leaf(f, table_schema.fields[(size_t)prune_cols[i]].name);
-            if (li < 0) continue;
+            if (li < 0 || f.leaves[(size_t)li].shape != pq::SHAPE_FLAT) continue;   // (list statistics bound the elements, not the rows)
             const int leaf_index = f.leaves[(size_t)li].leaf_index;
             if ((size_t)leaf_index >= rg.columns.size()) continue;
             const pq::ColumnMeta& cm = rg.columns[(size_t)leaf_index];
@@ -312,9 +335,9 @@ struct ParquetScanExec : Operator, FusedScanSource {
     }
     static int find_leaf(const FileState& f, const std::string& name) {
         for (size_t i = 0; i < f.leaves.size(); i++)
-            if (f.leaves[i].el.name == name) return (int)i;
+            if (f.leaves[i].name == name) return (int)i;
         for (size_t i = 0; i < f.leaves.size(); i++) {   // case-insensitive (scan/mod.rs:56-100)
-            const std::string& n = f.leaves[i].el.name;
+            const std::string& n = f.leaves[i].name;
             if (n.size() != name.size()) continue;
             bool eq = true;
             for (size_t k = 0; k < n.size(); k++) eq = eq && tolower(n[k]) == tolower(name[k]);
@@ -331,10 +354,12 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 continue;
             }
             int li = find_leaf(f, table_schema.fields[pj].name);
-            if (li < 0) s += "-;";
+            if (li < 0 || table_schema.fields[pj].type.id == T_NULL) s += "-;";
             else {
-                const pq::SchemaElement& el = f.leaves[li].el;   // (the annotation decides the conversion)
-                s += std::to_string(f.leaves[li].leaf_index) + ":" + std::to_string(el.type) + ":" + std::to_string(el.repetition) + ":" + std::to_string(el.type_length) +
+                const LeafColumn& lc = f.leaves[li];
+                const pq::SchemaElement& el = lc.el;   // (the annotation decides the conversion; a list's levels its layout)
+                s += std::to_string(lc.shape) + ":" + std::to_string(lc.max_def) + ":" + std::to_string(lc.list_def) + ":" + std::to_string(lc.elem_def) + ":" +
+                     std::to_string(f.leaves[li].leaf_index) + ":" + std::to_string(el.type) + ":" + std::to_string(el.repetition) + ":" + std::to_string(el.type_length) +
                      ":" + std::to_string(el.logical) + ":" + std::to_string(el.ts_unit) + ":" + std::to_string(el.int_bits) + ":" + std::to_string(el.int_signed) + ":" +
                      std::to_string(el.precision) + ":" + std::to_string(el.scale) + ";";
             }
@@ -363,6 +388,11 @@ struct ParquetScanExec : Operator, FusedScanSource {
         int64_t gpu_unc_bytes = 0;
         bool has_v1_inline = false;
         bool has_delta = false;   // some pages are DELTA_BINARY_PACKED: transcribed to PLAIN in the scratch buffer (pq_delta_to_plain)
+        // list columns: the level sections of every data page (slot_start local to the chunk; pointers of pages decompressed here are
+        // offsets into `unc` where levels_in_unc says so), and the chunk's level slots and non-null values
+        std::vector<PqLevelPage> levels;
+        std::vector<uint8_t> levels_in_unc;
+        int64_t n_slots = 0, n_vals = 0;
     };
     struct ChunkTask {
         std::shared_ptr<FileState> file;
@@ -396,6 +426,13 @@ struct ParquetScanExec : Operator, FusedScanSource {
         // bounds of the non-null values from the column-chunk statistics of every chunk in the batch (INT32 / INT64)
         bool stat_ok = true;
         int64_t stat_min = INT64_MAX, stat_max = INT64_MIN;
+        // the leaf's levels; a one-level list (shape SHAPE_LIST) decodes its element values as a required column of n_vals values
+        // (pages[].row_start = first value of the page) and its layout from `levels`
+        int shape = pq::SHAPE_FLAT;
+        int max_def = 0, max_rep = 0, list_def = 0, elem_def = 0;
+        std::string path;
+        std::vector<PqLevelPage> levels;
+        int64_t n_slots = 0, n_vals = 0;
     };
 
     // host-side count of non-null values of a v1 page (needed only for PLAIN string pages)
@@ -471,16 +508,24 @@ struct ParquetScanExec : Operator, FusedScanSource {
         return getenv("AURON_HOST_SNAPPY") == nullptr;   // AURON_HOST_SNAPPY=1: decompress on the host cores instead
     }
     // pure CPU: walk the pages of one column chunk (thread-safe, no CUDA calls)
-    static void parse_chunk(ChunkTask& ct, const pq::SchemaElement& el, bool is_string) {
+    static int bit_width(int v) {
+        int b = 0;
+        while ((1 << b) <= v) b++;
+        return b;
+    }
+    static void parse_chunk(ChunkTask& ct, const ColState& cs) {
+        const pq::SchemaElement& el = cs.el;
+        const bool is_string = cs.is_string;
         const pq::ColumnMeta& cm = *ct.cm;
         ChunkPages& out = ct.out;
         const uint8_t* host = ct.host;
         const uint8_t* dev = ct.dev;
         const int64_t len = cm.total_compressed;
-        const int max_def = el.repetition == 1 ? 1 : 0;
+        const bool is_list = cs.shape == pq::SHAPE_LIST;
+        const int max_def = is_list ? cs.max_def : el.repetition == 1 ? 1 : 0;
         const bool compressed = cm.codec != pq::CODEC_UNCOMPRESSED;
         const bool dev_snappy = cm.codec == pq::CODEC_SNAPPY && gpu_snappy();
-        int64_t pos = 0, values_seen = 0, rows = ct.row_start;
+        int64_t pos = 0, values_seen = 0, rows = is_list ? 0 : ct.row_start;   // (lists: rows counts values)
         int cur_dict = -1;
         while (pos < len && values_seen < cm.num_values) {
             pq::PageHeader h = pq::parse_page_header(host + pos, (size_t)(len - pos));
@@ -497,7 +542,9 @@ struct ParquetScanExec : Operator, FusedScanSource {
             // decompressed on the host (other codecs; and the one Snappy case whose levels the host must see: a PLAIN string
             // page needs its non-null count to place its values, which a nullable v1 page only has inside its body).
             const bool delta_strings = is_string && (h.encoding == pq::ENC_DELTA_LENGTH_BYTE_ARRAY || h.encoding == pq::ENC_DELTA_BYTE_ARRAY);
-            const bool page_dev = dev_snappy && !(is_string && h.type == pq::PAGE_DATA && h.encoding == pq::ENC_PLAIN && max_def > 0) && !delta_strings;
+            // (the levels of a v1 list page are inside its body: the host counts the page's values from them, so it decompresses the body)
+            const bool page_dev = dev_snappy && !(is_string && h.type == pq::PAGE_DATA && h.encoding == pq::ENC_PLAIN && max_def > 0) && !delta_strings &&
+                                  !(is_list && h.type == pq::PAGE_DATA);
             bool on_device = false;
             int64_t gap = 0;   // stored v2 page with level sections: Snappy framing bytes between the levels and the values
             if (page_compressed && page_dev) {
@@ -592,7 +639,35 @@ struct ParquetScanExec : Operator, FusedScanSource {
             }
             int64_t o = 0, total = h.uncompressed_size;
             int32_t delta_nn = -1;   // non-null values of a delta-encoded string page (its streams say so)
-            if (h.type == pq::PAGE_DATA) {
+            int32_t list_nn = -1;    // list pages: the page's non-null values
+            int64_t rep_off = 0, def_off = 0;   // list pages: level sections (offsets in the page body)
+            PqLevelPage lv{};
+            if (is_list) {
+                lv.n_slots = h.num_values;
+                if (h.type == pq::PAGE_DATA) {   // [u32 length][repetition levels][u32 length][definition levels][values]
+                    AURON_CHECK(h.rep_encoding == pq::ENC_RLE && h.def_encoding == pq::ENC_RLE, "only RLE repetition and definition levels are supported (column " + cs.path + ")");
+                    uint32_t rl = 0, dl = 0;
+                    AURON_CHECK(total >= 8, "corrupt parquet list page (column " + cs.path + ")");
+                    memcpy(&rl, hp(0), 4);
+                    AURON_CHECK((int64_t)rl + 8 <= total, "corrupt parquet list page levels (column " + cs.path + ")");
+                    memcpy(&dl, hp(4 + (int64_t)rl), 4);
+                    AURON_CHECK((int64_t)rl + 8 + (int64_t)dl <= total, "corrupt parquet list page levels (column " + cs.path + ")");
+                    rep_off = 4;
+                    def_off = 8 + (int64_t)rl;
+                    lv.rep_len = (int32_t)rl;
+                    lv.def_len = (int32_t)dl;
+                    o = def_off + dl;
+                    list_nn = (int32_t)pq::hybrid_count(hp(def_off), dl, bit_width(max_def), h.num_values, (uint32_t)max_def);
+                } else {   // v2: levels stored uncompressed in front of the values, the header counts the NULL slots
+                    AURON_CHECK(h.rep_bytes >= 0 && h.def_bytes >= 0 && (int64_t)h.rep_bytes + h.def_bytes <= total && h.num_nulls >= 0 && h.num_nulls <= h.num_values,
+                                "corrupt parquet list page levels (column " + cs.path + ")");
+                    def_off = h.rep_bytes;
+                    lv.rep_len = h.rep_bytes;
+                    lv.def_len = h.def_bytes;
+                    o = (int64_t)h.rep_bytes + h.def_bytes;
+                    list_nn = h.num_values - h.num_nulls;
+                }
+            } else if (h.type == pq::PAGE_DATA) {
                 if (max_def > 0) {
                     AURON_CHECK(h.def_encoding == pq::ENC_RLE, "only RLE definition levels are supported");
                     pg.def_ptr = (const uint8_t*)(intptr_t)4;   // offsets now, pointers once the base is known
@@ -624,6 +699,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 const std::vector<uint8_t> head(hp(0), hp(0) + o);
                 int32_t nn = 0;
                 const std::vector<uint8_t> plain = delta_strings_to_plain(hp(o + gap), (size_t)(total - o - gap), h.encoding == pq::ENC_DELTA_BYTE_ARRAY, &nn, (size_t)h.num_values);
+                AURON_CHECK(list_nn < 0 || nn == list_nn, "corrupt parquet list page: its values do not match its levels (column " + cs.path + ")");
                 unc_off = (int64_t)out.unc.size();
                 out.unc.resize(out.unc.size() + head.size() + plain.size() + 8);
                 if (!head.empty()) memcpy(out.unc.data() + unc_off, head.data(), head.size());
@@ -645,17 +721,64 @@ struct ParquetScanExec : Operator, FusedScanSource {
             size_t sec_idx = SIZE_MAX;
             if (is_string && pg.encoding == pq::ENC_PLAIN) {
                 // PLAIN string pages need their exact non-null count: v2 gives it, v1 requires the def levels
-                int32_t nn = delta_nn >= 0 ? delta_nn : h.type == pq::PAGE_DATA_V2 ? h.num_values - h.num_nulls : count_non_null_v1(hp(0), max_def, h.num_values);
+                int32_t nn = delta_nn >= 0 ? delta_nn : list_nn >= 0 ? list_nn : h.type == pq::PAGE_DATA_V2 ? h.num_values - h.num_nulls : count_non_null_v1(hp(0), max_def, h.num_values);
                 pg.plain_value_base = (int32_t)out.value_table_size;
                 sec_idx = out.secs.size();
                 out.secs.push_back({base_d ? pg.val_ptr : nullptr, pg.val_len, nn, (int32_t)out.value_table_size});
                 out.value_table_size += nn;
             }
+            if (is_list) {
+                // the values decode as a required column: the page holds list_nn of them, placed behind those of the pages before it
+                pg.num_values = list_nn;
+                // v2 levels are never compressed: they are read where the chunk lies; v1 levels from the page body, in place or in `unc`
+                const bool in_unc = h.type == pq::PAGE_DATA && unc_off >= 0;
+                const uint8_t* lbase = in_unc ? (const uint8_t*)(intptr_t)unc_off : h.type == pq::PAGE_DATA ? payload_d : dev + (pos - h.compressed_size);
+                lv.rep = lbase + rep_off;
+                lv.def = lbase + def_off;
+                lv.slot_start = (int32_t)out.n_slots;
+                AURON_CHECK(out.n_slots + h.num_values <= (int64_t)INT32_MAX, "parquet list column " + cs.path + ": a column chunk of more than 2^31 - 1 level slots");
+                out.levels.push_back(lv);
+                out.levels_in_unc.push_back(in_unc ? 1 : 0);
+                out.n_slots += h.num_values;
+                out.n_vals += list_nn;
+            }
             if (unc_off >= 0) out.fixes.push_back({out.pages.size(), 0, sec_idx, unc_off, on_device});
             out.pages.push_back(pg);
-            rows += h.num_values;
+            rows += is_list ? list_nn : h.num_values;
             values_seen += h.num_values;
         }
+    }
+
+    // the column state of a projected field that the file holds: its shape must be one the table type can read
+    static void check_shape(const LeafColumn& lc, const Field& fld) {
+        const bool want_list = fld.type.id == T_LIST;
+        if (lc.shape == pq::SHAPE_FLAT && want_list)
+            fail("cannot read parquet column " + lc.name + " (a primitive column, physical type " + std::to_string(lc.el.type) + ") as " + fld.type.str());
+        if (lc.shape == pq::SHAPE_LIST && !want_list)
+            fail("cannot read parquet column " + lc.name + " (a list of physical type " + std::to_string(lc.el.type) + ") as " + fld.type.str());
+        if (lc.shape != pq::SHAPE_FLAT && lc.shape != pq::SHAPE_LIST)
+            fail("cannot read parquet column " + lc.name + " (a " + pq::shape_name(lc.shape) + "): only primitive columns and lists of primitives are read");
+    }
+    static void setup_column(ColState& cs, const LeafColumn& lc, const Field& fld) {
+        check_shape(lc, fld);
+        AURON_CHECK(lc.leaf_index >= 0, "parquet column " + lc.name + " has no leaf");
+        cs.el = lc.el;
+        cs.shape = lc.shape;
+        cs.path = lc.path;
+        cs.max_def = lc.max_def;
+        cs.max_rep = lc.max_rep;
+        cs.list_def = lc.list_def;
+        cs.elem_def = lc.elem_def;
+        if (lc.shape == pq::SHAPE_LIST) {
+            AURON_CHECK(fld.type.elem && fld.type.elem->id != T_LIST, "list column " + fld.name + " without a flat element type");
+            AURON_CHECK(lc.max_rep == 1 && lc.max_def >= lc.elem_def && lc.max_def <= lc.elem_def + 1, "parquet column " + lc.name + ": unexpected list levels");
+            pq::SchemaElement e = lc.el;
+            e.name = lc.path;   // (a conversion error names the column and its element)
+            cs.cv = conversion_of(e, *fld.type.elem);
+        } else {
+            cs.cv = conversion_of(lc.el, fld.type);
+        }
+        cs.is_string = lc.el.type == pq::PT_BYTE_ARRAY;
     }
 
     static int phys_width(int phys, int type_length) {
@@ -852,6 +975,92 @@ struct ParquetScanExec : Operator, FusedScanSource {
             l->kernel_launches = 0;
         }
     }
+    // every row a NULL list: zero offsets, a clear validity bitmap and an empty child of the element type (a file without the column)
+    static ColumnPtr null_list_column(Ctx& ctx, const DType& t, int64_t n_rows) {
+        auto col = std::make_shared<Column>();
+        col->type = t;
+        col->len = n_rows;
+        col->offsets = dalloc_zero(ctx, (size_t)(n_rows + 1) * 4);
+        col->validity = dalloc_zero(ctx, bitmap_alloc_bytes(n_rows));
+        col->null_count = n_rows;
+        col->child = make_column(ctx, *t.elem, 0, false);
+        return col;
+    }
+    // A one-level list column of the batch (on the task stream): the element values of every page decode as one required column,
+    // the level pass (k_parquet_levels.cu) gives the offsets, the list validity and each element's value, one gather places the values.
+    ColumnPtr build_list_column(Task& t, ColState& cs, const Field& fld, int64_t n_rows) {
+        const DType& et = *fld.type.elem;
+        const pq::SchemaElement& el = cs.el;
+        const int64_t nv = cs.n_vals;
+        AURON_CHECK(nv <= cs.n_slots, "corrupt parquet list column " + cs.path + ": more values than level slots");
+        Buf dpages = to_device(t.ctx, cs.pages.empty() ? (const void*)"" : (const void*)cs.pages.data(), cs.pages.size() * sizeof(PqPage));
+        Buf ddicts = to_device(t.ctx, cs.dicts.empty() ? (const void*)"" : (const void*)cs.dicts.data(), cs.dicts.size() * sizeof(PqDict));
+        if (cs.has_delta) pq_delta_to_plain(t.ctx, P<PqPage>(dpages), (int)cs.pages.size(), unc_scratch_ptr, el.type == pq::PT_INT32 ? 4 : 8, status_ptr);
+        PqColumnArgs a;
+        memset(&a, 0, sizeof(a));
+        a.pages = P<PqPage>(dpages);
+        a.dicts = P<PqDict>(ddicts);
+        a.n_pages = (int)cs.pages.size();
+        a.phys_type = el.type;
+        a.type_length = el.type_length;
+        a.phys_width = phys_width(el.type, el.type_length);
+        a.out_type = et.id;
+        a.out_width = et.width();
+        a.out_unit = et.unit;
+        a.conv = cs.cv.kind;
+        a.conv_mul = cs.cv.mul;
+        a.conv_mul_hi = cs.cv.mul_hi;
+        a.max_def = 0;   // the values of a list page have no gaps
+        ColumnPtr vals;   // fixed-width: the values; strings: the value table, gathered once through str_idx below
+        Buf str_idx;      // strings: value -> entry of the value table
+        if (cs.is_string) {
+            vals = pq_build_value_table(t.ctx, cs.secs, cs.value_table_size, et);
+            str_idx = dalloc(t.ctx, (size_t)std::max<int64_t>(nv, 1) * 4);
+            a.mode = PQ_MODE_INDEX;
+            a.out_idx = P<int32_t>(str_idx);
+            if (!cs.pages.empty()) pq_decode_pages(t.ctx, a, cs.pages);
+        } else {
+            vals = std::make_shared<Column>();
+            vals->type = et;
+            vals->len = nv;
+            vals->data = et.id == T_BOOL ? dalloc_zero(t.ctx, bitmap_alloc_bytes(nv)) : dalloc(t.ctx, (size_t)std::max<int64_t>(nv, 1) * et.width());
+            if (cs.cv.kind == PQ_CV_TS_MUL) {   // (overflowing products are NULL)
+                vals->validity = dalloc_zero(t.ctx, bitmap_alloc_bytes(nv));
+                vals->null_count = -1;
+            }
+            a.mode = PQ_MODE_VALUES;
+            a.out = vals->data->ptr;
+            a.out_valid = P<uint32_t>(vals->validity);
+            if (!cs.pages.empty()) pq_decode_pages(t.ctx, a, cs.pages);
+        }
+        PqListShape sh;
+        sh.rep_bw = bit_width(cs.max_rep);
+        sh.def_bw = bit_width(cs.max_def);
+        sh.list_def = cs.list_def;
+        sh.elem_def = cs.elem_def;
+        sh.max_def = cs.max_def;
+        auto col = std::make_shared<Column>();
+        col->type = fld.type;
+        col->len = n_rows;
+        col->offsets = dalloc(t.ctx, (size_t)(n_rows + 1) * 4);
+        if (cs.list_def > 0) {
+            col->validity = dalloc_zero(t.ctx, bitmap_alloc_bytes(n_rows));
+            col->null_count = -1;
+        }
+        Buf elem_idx = dalloc(t.ctx, (size_t)std::max<int64_t>(cs.n_slots, 1) * 4);
+        Buf counts = dalloc(t.ctx, 4 * sizeof(int64_t));
+        Buf dlevels = to_device(t.ctx, cs.levels.empty() ? (const void*)"" : (const void*)cs.levels.data(), cs.levels.size() * sizeof(PqLevelPage));
+        pq_list_levels(t.ctx, P<PqLevelPage>(dlevels), (int)cs.levels.size(), cs.n_slots, n_rows, sh, P<int32_t>(col->offsets), P<uint32_t>(col->validity),
+                       P<int32_t>(elem_idx), P<int64_t>(counts));
+        int64_t c[4];
+        to_host(t.ctx, c, counts->ptr, sizeof(c));   // (the element count sizes the gather)
+        AURON_CHECK(c[3] == 0, "corrupt parquet list column " + cs.path + ": malformed levels in page " + std::to_string(c[3] - 1) + " of the batch");
+        AURON_CHECK(c[0] == n_rows && c[2] == nv, "corrupt parquet list column " + cs.path + ": the levels hold " + std::to_string(c[0]) + " rows and " +
+                                                       std::to_string(c[2]) + " values, the pages " + std::to_string(n_rows) + " and " + std::to_string(nv));
+        if (str_idx) pq_compose_index(t.ctx, P<int32_t>(elem_idx), P<int32_t>(str_idx), c[1]);   // element -> value-table entry
+        col->child = take(t.ctx, *vals, P<int32_t>(elem_idx), c[1], cs.max_def > cs.elem_def);
+        return col;
+    }
     BatchPtr build_batch(Task& t, std::vector<ColState>& cols, int64_t n_rows, const std::vector<FileSeg>& file_segs) {
         AURON_CHECK(n_rows < (int64_t)INT32_MAX, "parquet batch too large");
         auto out = std::make_shared<Batch>();
@@ -896,12 +1105,19 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 continue;
             }
             if (cs.leaf < 0) {   // missing column -> NULL (scan/mod.rs:84-100)
-                if (fld.type.is_varlen()) {
+                if (fld.type.id == T_LIST) {
+                    out->cols.push_back(null_list_column(t.ctx, fld.type, n_rows));
+                } else if (fld.type.is_varlen()) {
                     auto c = make_column(t.ctx, fld.type, n_rows, true);
                     c->null_count = n_rows;
                     CUDA_OK(cudaMemsetAsync(c->offsets->ptr, 0, (size_t)(n_rows + 1) * 4, t.ctx.stream));
                     out->cols.push_back(c);
                 } else out->cols.push_back(make_null_column(t.ctx, fld.type, n_rows));
+                continue;
+            }
+            if (cs.shape == pq::SHAPE_LIST) {
+                if (cs.needs_decomp && decomp_done) CUDA_OK(cudaStreamWaitEvent(t.ctx.stream, decomp_done, 0));
+                out->cols.push_back(build_list_column(t, cs, fld, n_rows));
                 continue;
             }
             const pq::SchemaElement& el = cs.el;
@@ -1078,16 +1294,18 @@ struct ParquetScanExec : Operator, FusedScanSource {
                     }
                     const Field& fld = table_schema.fields[projection[ci]];
                     int li = find_leaf(*cur, fld.name);
+                    if (fld.type.id == T_NULL) li = -1;   // a field the query does not read (NullType): NULL, whatever the file holds
                     p.cols[ci].leaf = li;
                     if (li < 0) continue;
-                    p.cols[ci].el = cur->leaves[li].el;
-                    p.cols[ci].cv = conversion_of(p.cols[ci].el, fld.type);
-                    p.cols[ci].is_string = p.cols[ci].el.type == pq::PT_BYTE_ARRAY;
+                    setup_column(p.cols[ci], cur->leaves[(size_t)li], fld);
                 }
             }
             for (size_t ci = 0; ci < projection.size(); ci++) {
                 if (p.cols[ci].leaf < 0) continue;
-                int leaf_index = cur->leaves[find_leaf(*cur, table_schema.fields[projection[ci]].name)].leaf_index;
+                // (by name in THIS file: field positions differ between files whose signatures match)
+                const int li = find_leaf(*cur, table_schema.fields[projection[ci]].name);
+                AURON_CHECK(li >= 0, "parquet column " + table_schema.fields[projection[ci]].name + " missing from a row group of its batch");
+                int leaf_index = cur->leaves[(size_t)li].leaf_index;
                 AURON_CHECK((size_t)leaf_index < rg.columns.size(), "row group misses a column chunk");
                 ChunkTask ct;
                 ct.file = cur;
@@ -1195,7 +1413,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
             CUDA_OK(cudaEventRecord(p.copied, copy_stream));
         }
         auto t1 = std::chrono::steady_clock::now();
-        parallel_for(p.tasks.size(), host_threads, [&](size_t i) { parse_chunk(p.tasks[i], p.cols[p.tasks[i].col].el, p.cols[p.tasks[i].col].is_string); });
+        parallel_for(p.tasks.size(), host_threads, [&](size_t i) { parse_chunk(p.tasks[i], p.cols[p.tasks[i].col]); });
         auto t2 = std::chrono::steady_clock::now();
         p.fetch_ns = std::chrono::duration_cast<std::chrono::nanoseconds>(t1 - t0).count();
         p.parse_ns = std::chrono::duration_cast<std::chrono::nanoseconds>(t2 - t1).count();
@@ -1357,6 +1575,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
         // device-decompressed pages and in the job list; value bounds from the chunk statistics.
         struct Slot {
             int64_t unc_off = 0;
+            int64_t val_base = 0;   // list columns: the chunk's first value within the batch
             size_t job_base = 0, page_base = 0, dict_base = 0, sec_base = 0;
             int32_t vbase = 0;
             Buf host_unc;   // chunks decompressed on the host: their payload, uploaded below
@@ -1400,6 +1619,22 @@ struct ParquetScanExec : Operator, FusedScanSource {
             if (!cp.unc.empty()) {   // host-decompressed payloads (ZSTD / LZ4_RAW pages, nullable v1 PLAIN string pages) are uploaded here
                 sl.host_unc = to_device(wc, cp.unc.data(), cp.unc.size());
                 cs.keep.push_back(sl.host_unc);
+            }
+            if (cs.shape == pq::SHAPE_LIST) {   // level sections, rebased to the batch (a few descriptors per page: serial)
+                AURON_CHECK(cs.n_slots + cp.n_slots <= (int64_t)INT32_MAX,
+                            "parquet list column " + cs.path + ": a batch of more than 2^31 - 1 list elements and empty or NULL lists; lower AURON_GPU_CHUNK_ROWS");
+                sl.val_base = cs.n_vals;
+                for (size_t i = 0; i < cp.levels.size(); i++) {
+                    PqLevelPage lv = cp.levels[i];
+                    lv.slot_start += (int32_t)cs.n_slots;
+                    if (cp.levels_in_unc[i]) {
+                        lv.rep = P<uint8_t>(sl.host_unc) + (intptr_t)lv.rep;
+                        lv.def = P<uint8_t>(sl.host_unc) + (intptr_t)lv.def;
+                    }
+                    cs.levels.push_back(lv);
+                }
+                cs.n_slots += cp.n_slots;
+                cs.n_vals += cp.n_vals;
             }
         }
         uint8_t* unc_scratch = nullptr;   // one scratch block for every device-decompressed page of the batch
@@ -1464,6 +1699,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 if (pg.dict_id >= 0) pg.dict_id += (int32_t)sl.dict_base;
                 if (pg.delta_dst16) pg.delta_dst16 += (int32_t)(sl.unc_off / 16);
                 pg.plain_value_base += sl.vbase;
+                if (cs.shape == pq::SHAPE_LIST) pg.row_start += (int32_t)sl.val_base;
                 dst[i] = pg;
             }
         });
@@ -2027,6 +2263,8 @@ OperatorPtr make_parquet_scan(Task& t, const uint8_t* node, size_t n) {
     for (int p : op->projection) {
         AURON_CHECK(p >= 0 && p < (int)(op->table_schema.fields.size() + op->part_schema.fields.size()), "scan projection out of range");
         op->out_schema.fields.push_back(op->proj_field(p));
+        const Field& f = op->proj_field(p);
+        if (f.type.id == T_LIST && op->is_part_col(p)) fail("ParquetScanExec: list column " + f.name + " (" + f.type.str() + ") is not supported as a partition column");
     }
     (void)t;
     return op;

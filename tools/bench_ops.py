@@ -3,6 +3,7 @@ time per launch site from the library's CUDA-event timers (AURON_PROFILE=1).  Th
 north star asks for next to the config-2 bench line; they are not bench.py lines.
 
     python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [scalar] [casts] [window] [generate]
+                              [parquet_list]
 
   join     cfg 3: store_sales (N rows: ss_sold_date_sk int32, ss_item_sk int32, ss_quantity int32) JOIN date_dim (73,049 rows:
            d_date_sk int32, d_year int32) on the date key, inner, build = date_dim
@@ -29,6 +30,11 @@ north star asks for next to the config-2 bench line; they are not bench.py lines
   generate LATERAL VIEW explode(split(s, ',')) + COUNT grouped by the element over N rows of 34 B strings (five 6-letter words from a
            vocabulary of 1,000, four separators), in device batches of 16M rows.  Reports the device time of the split kernels and of
            the generate gather with their algorithmic bytes, then the Filter -> Project leg, so that both come from the same run
+  parquet_list  Parquet scan of N rows of list<int64> and of list<string> (0-8 elements, mean 4; 5 % NULL elements; SNAPPY; data
+           page v1 and v2) -> explode -> COUNT.  Reports the device time of the level pass (pq_list_levels) next to the whole pass,
+           then the config-2 fused leg (SNAPPY Parquet of N rows item / qty / date int32 -> Filter -> partial SUM / COUNT by item,
+           best of 5 passes) and the Filter -> Project leg three times each, each time followed by the same leg of the built checkout
+           at $OPS_PARENT when that is set
 """
 import os
 import sys
@@ -438,3 +444,83 @@ if "generate" in which:
         alg={"string_split": split_b, "take": take_b})
     runtime.drop_device_resource("gen")
     filter_project_leg()
+
+if "parquet_list" in which:
+    import subprocess
+    import tempfile
+
+    import pyarrow.parquet as pq
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"== parquet_list leg on: {gpu}")
+    U = pa.string()
+    lens = rng.integers(0, 9, N).astype(np.int32)
+    offs = np.zeros(N + 1, dtype=np.int32)
+    np.cumsum(lens, out=offs[1:])
+    n_el = int(offs[-1])
+    mask = rng.random(n_el) < 0.05
+    vocab = np.array([f"tag{i:05d}" for i in range(10_000)], dtype=object)
+    with tempfile.TemporaryDirectory() as d:
+        for kind in ("int64", "string"):
+            if kind == "int64":
+                child = pa.array(rng.integers(-2**40, 2**40, n_el), pa.int64(), mask=mask)
+            else:
+                words = vocab[rng.integers(0, len(vocab), n_el)]
+                child = pa.array(words, U, mask=mask)
+            col = pa.ListArray.from_arrays(pa.array(offs), child)
+            tab = pa.table({"l": col})
+            for ver in ("1.0", "2.0"):
+                path = os.path.join(d, f"{kind}_{ver}.parquet")
+                pq.write_table(tab, path, compression="SNAPPY", data_page_version=ver, row_group_size=4 << 20)
+                scan = P.parquet_scan(tab.schema, [(path, os.path.getsize(path))], [0])
+                gen = P.generate(scan, "Explode", P.col("l"), [], [("w", tab.schema.field("l").type.value_type, True)])
+                plan = P.agg(gen, [], [], [P.agg_expr("COUNT", [P.col("w")], pa.int64())], ["c"], ["PARTIAL"])
+                with runtime.Task(P.task_definition(plan)) as task:
+                    got = sum(sum(b.column(0).to_pylist()) for b in task)
+                assert got == n_el - int(mask.sum()), got
+                run(plan, f"parquet list<{kind}> v{ver} SNAPPY ({os.path.getsize(path) >> 20} MiB) -> explode -> COUNT over {N} rows, {n_el} elements", N,
+                    steps=3)
+                os.remove(path)
+        # the config-2 fused leg, run in a fresh process from a tree's root (this one, then the parent's), the same file for both
+        fused = os.path.join(d, "cfg2.parquet")
+        pq.write_table(pa.table({"item": pa.array(rng.integers(1, 204001, N).astype(np.int32)),
+                                 "qty": pa.array(rng.integers(1, 101, N).astype(np.int32), mask=rng.random(N) < 0.03),
+                                 "date": pa.array(rng.integers(2450816, 2452642, N).astype(np.int32), mask=rng.random(N) < 0.04)}),
+                       fused, compression="SNAPPY", row_group_size=8 << 20)
+        leg = """
+import os, sys, time
+sys.path.insert(0, os.getcwd())
+import pyarrow as pa
+from auron_b200 import proto as P
+from auron_b200 import runtime
+path = sys.argv[1]
+I32, I64 = pa.int32(), pa.int64()
+sch = pa.schema([("item", I32), ("qty", I32), ("date", I32)])
+flt = P.filter_(P.parquet_scan(sch, [(path, os.path.getsize(path))], [0, 1, 2]),
+                [P.binary("GtEq", P.col("date"), P.lit(2451000, I32)), P.binary("Lt", P.col("date"), P.lit(2452000, I32))])
+plan = P.agg(flt, [P.try_cast(P.col("item"), I64)], ["item"], [P.agg_expr("SUM", [P.col("qty")], I64), P.agg_expr("COUNT", [P.col("qty")], I64)],
+             ["s", "c"], ["PARTIAL", "PARTIAL"])
+best, fused = None, 0
+for _ in range(5):
+    t0 = time.perf_counter()
+    with runtime.Task(P.task_definition(plan)) as task:
+        rows = sum(b.num_rows for b in task)
+        fused = sum(v for _, _, n, v in task.metrics() if n == "fused_batches")
+    dt = time.perf_counter() - t0
+    best = dt if best is None else min(best, dt)
+print(f"fused_ms {1000 * best:.1f} groups {rows} fused_batches {fused}")
+"""
+        here = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+        parent = os.environ.get("OPS_PARENT")
+        for k in range(3):
+            for label, root in [("this tree", here)] + ([("parent tree", parent)] if parent else []):
+                out = subprocess.run([sys.executable, "-c", leg, fused], capture_output=True, text=True, cwd=root).stdout.strip()
+                print(f"== config-2 fused leg over {N} rows, {label}, pass {k + 1}: {out}")
+    for k in range(3):
+        print(f"== Filter -> Project, this tree, pass {k + 1}: expr_vm {filter_project_leg().get('expr_vm', 0) / 1000:.3f} ms")
+        if parent:
+            import re
+            out = subprocess.run([sys.executable, os.path.join(parent, "tools", "bench_ops.py"), "filter_project"], capture_output=True, text=True,
+                                 cwd=parent, env=dict(os.environ, OPS_ROWS=str(N))).stdout
+            ms = re.search(r"expr_vm\s+([0-9.]+) ms", out)
+            print(f"== Filter -> Project, parent tree, pass {k + 1}: expr_vm {ms.group(1) if ms else '?'} ms")
