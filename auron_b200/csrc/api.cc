@@ -222,6 +222,18 @@ int auron_b200_text_to_float(int32_t bits, const uint8_t* text, int64_t len, uin
     API_GUARD_END(-1)
 }
 
+int64_t auron_b200_zstd_decompress(const uint8_t* in, int64_t in_len, uint8_t* out, int64_t out_len) {
+    API_GUARD_BEGIN
+    if (in_len < 0 || out_len < 0 || (in_len > 0 && !in) || (out_len > 0 && !out)) {
+        g_last_error = "zstd_decompress: lengths must be >= 0 and buffers non-null";
+        return -1;
+    }
+    const int64_t r = zstd_decompress_host(in, in_len, out, out_len);
+    if (r < 0) g_last_error = "zstd_decompress: malformed ZSTD data, or more than out_len bytes";
+    return r;
+    API_GUARD_END(-1)
+}
+
 // ---- device residency
 static std::map<int, std::unique_ptr<Ctx>>& util_ctxs() {
     static std::map<int, std::unique_ptr<Ctx>> m;

@@ -568,25 +568,27 @@ __global__ void pq_fix_v1_pages_kernel(PqPage* __restrict__ pages, int n, const 
     pages[i] = pg;
 }
 
-PqDecompOut pq_decompress(Ctx& ctx, const std::vector<PqDecompJob>& jobs) {
+PqDecompOut pq_decompress(Ctx& ctx, const std::vector<PqDecompJob>& jobs, size_t n_snappy) {
     PqDecompOut out;
     out.status = dalloc_zero(ctx, 4);
     if (jobs.empty()) return out;
     out.results = dalloc(ctx, jobs.size() * sizeof(PqDecompResult));
     Buf dj = to_device(ctx, jobs.data(), jobs.size() * sizeof(PqDecompJob));
-    Buf states = dalloc(ctx, jobs.size() * sizeof(PqDecompState));
+    pq_decompress_zstd_lz4(ctx, jobs, n_snappy, P<PqDecompJob>(dj), P<int32_t>(out.status), P<PqDecompResult>(out.results));
+    if (n_snappy == 0) return out;
+    Buf states = dalloc(ctx, n_snappy * sizeof(PqDecompState));
     ProfScope ps(ctx, "pq_decompress");
     // AURON_SNAPPY_THREADS=1: the one-thread-per-job prefix pass.  A thread alone pays the full shared-memory latency per byte
     // (load, store, next byte); the four-lane teams overlap four bytes and eight streams per warp.  Kept selectable as the alternative.
     static const bool teams = getenv("AURON_SNAPPY_THREADS") == nullptr;
     if (teams)
-        pq_decompress_prefix_kernel<<<(unsigned)((jobs.size() + 4 * SN_TEAMS - 1) / (4 * SN_TEAMS)), 128, 0, ctx.stream>>>(P<PqDecompJob>(dj), (int)jobs.size(), P<int32_t>(out.status),
+        pq_decompress_prefix_kernel<<<(unsigned)((n_snappy + 4 * SN_TEAMS - 1) / (4 * SN_TEAMS)), 128, 0, ctx.stream>>>(P<PqDecompJob>(dj), (int)n_snappy, P<int32_t>(out.status),
                                                                                                      P<PqDecompResult>(out.results), P<PqDecompState>(states));
     else
-        pq_decompress_thread_kernel<<<(unsigned)((jobs.size() + 63) / 64), 64, 0, ctx.stream>>>(P<PqDecompJob>(dj), (int)jobs.size(), P<int32_t>(out.status),
+        pq_decompress_thread_kernel<<<(unsigned)((n_snappy + 63) / 64), 64, 0, ctx.stream>>>(P<PqDecompJob>(dj), (int)n_snappy, P<int32_t>(out.status),
                                                                                                    P<PqDecompResult>(out.results), P<PqDecompState>(states));
     LAUNCH_CHECK(ctx);
-    pq_decompress_kernel<<<(unsigned)((jobs.size() + 3) / 4), 128, 0, ctx.stream>>>(P<PqDecompJob>(dj), (int)jobs.size(), P<int32_t>(out.status),
+    pq_decompress_kernel<<<(unsigned)((n_snappy + 3) / 4), 128, 0, ctx.stream>>>(P<PqDecompJob>(dj), (int)n_snappy, P<int32_t>(out.status),
                                                                                        P<PqDecompResult>(out.results), P<PqDecompState>(states));
     LAUNCH_CHECK(ctx);
     return out;

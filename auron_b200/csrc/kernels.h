@@ -74,6 +74,8 @@ int digest_hex_host(int alg, const uint8_t* bytes, int64_t len, char* out);
 // (float_text.cuh, the code the device runs).  bits: 32 or 64; values are bit patterns.
 int float_to_text_host(int bits, uint64_t value, char* out);   // Java's Float / Double.toString into out (>= 24 bytes); the length
 bool text_to_float_host(int bits, const uint8_t* text, int32_t len, uint64_t* value);   // Spark's CAST; false: NULL
+// k_zstd.cu: the device's ZSTD page decoder (zstd_dec.cuh) on the CPU; bytes written into out[0, out_len), or -1 (malformed or too long)
+int64_t zstd_decompress_host(const uint8_t* in, int64_t in_len, uint8_t* out, int64_t out_len);
 
 // ----------------------------------------------------------------------------- k_rowkeys.cu
 // Row-key view over key columns for hash aggregation / joins (general path)

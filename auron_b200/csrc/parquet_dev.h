@@ -65,7 +65,8 @@ struct PqDecompJob {
     uint8_t* dst;
     int32_t src_len, dst_len;
     int32_t kind;       // 0 = stored bytes, 1 = Snappy raw block, 2 = the front elements of a Snappy raw block (the preamble
-                        //     counts the whole block; the job ends after src_len bytes, which decode to dst_len bytes)
+                        //     counts the whole block; the job ends after src_len bytes, which decode to dst_len bytes),
+                        //     3 = ZSTD frames, 4 = LZ4 raw block (PqJobKind)
     int32_t v1_levels;  // 1 = body of a nullable v1 data page ([u32 length][levels][values]): a final literal that holds the
                         //     whole value section is NOT copied, the page then reads its values from the compressed buffer
 };
@@ -78,7 +79,11 @@ struct PqDecompOut {
     Buf status;    // int32: 0 = ok, else 1 + index of the first failing job
     Buf results;   // PqDecompResult per job
 };
-PqDecompOut pq_decompress(Ctx& ctx, const std::vector<PqDecompJob>& jobs);
+enum PqJobKind { PQ_JOB_STORED = 0, PQ_JOB_SNAPPY = 1, PQ_JOB_SNAPPY_HEAD = 2, PQ_JOB_ZSTD = 3, PQ_JOB_LZ4 = 4 };
+// jobs[0, n_snappy) are stored / Snappy jobs (k_snappy.cu), jobs[n_snappy, size) stored / ZSTD / LZ4_RAW jobs (k_zstd.cu)
+PqDecompOut pq_decompress(Ctx& ctx, const std::vector<PqDecompJob>& jobs, size_t n_snappy);
+void pq_decompress_zstd_lz4(Ctx& ctx, const std::vector<PqDecompJob>& jobs, size_t first, const PqDecompJob* dev_jobs, int32_t* status,
+                            PqDecompResult* results);
 // pages with def_len == -1: level / value sections from the body's length word (+ in-place value sections, see above)
 void pq_fix_v1_pages(Ctx& ctx, PqPage* pages, int n, const PqDecompResult* results);
 // pages with delta_dst16 != 0: DELTA_BINARY_PACKED values (width 4 or 8 bytes) -> PLAIN values at scratch + 16 (delta_dst16 - 1);

@@ -8,8 +8,10 @@
 //   2. fetch  : HBM-resident file images are used in place; host files are pread by a thread pool into one pinned
 //               staging buffer and uploaded with a single async copy
 //   3. parse  : page headers of every chunk (Thrift) in parallel on host threads -> page / dictionary descriptors and the list of
-//               device decompression jobs (SNAPPY: k_snappy.cu; large literal chains are split into stored-copy jobs here, tags
-//               only); ZSTD / LZ4_RAW pages are decompressed on the host cores, UNCOMPRESSED pages are decoded in place;
+//               device decompression jobs (SNAPPY: k_snappy.cu, large literal chains are split into stored-copy jobs here, tags
+//               only; ZSTD and LZ4_RAW: k_zstd.cu, one job per page body); the pages whose body the host must see are decompressed
+//               on the host cores (nullable v1 PLAIN string pages, delta-encoded string pages, v1 list pages), UNCOMPRESSED pages
+//               are decoded in place;
 //               delta-encoded string pages are rewritten as PLAIN, Hive partition columns become constant columns, row groups
 //               that the pruning predicates exclude by their statistics are skipped at plan time
 //   4. decode : k_parquet.cu, one scout launch for all columns + one decode launch per column -- or, when the plan above is
@@ -382,10 +384,12 @@ struct ParquetScanExec : Operator, FusedScanSource {
             bool dev;      // off is relative to the device scratch (decompressed by the GPU), else to `unc` (decompressed here)
         };
         std::vector<Fix> fixes;
-        // SNAPPY pages are decompressed on the device (all but nullable v1 PLAIN string pages): jobs with dst as an OFFSET into a scratch
+        // SNAPPY, ZSTD and LZ4_RAW pages are decompressed on the device (all but the pages the host must see): jobs with dst as an OFFSET into a scratch
         // buffer of gpu_unc_bytes that the task thread allocates; `fixes` then patch the descriptors with the scratch base
         std::vector<PqDecompJob> jobs;
+        bool snappy_jobs = true;   // jobs for k_snappy.cu, else for k_zstd.cu (ZSTD / LZ4_RAW chunks)
         int64_t gpu_unc_bytes = 0;
+        int64_t pages_dev = 0, pages_host = 0;   // compressed pages (dictionary and data) decompressed on the device / on the host
         bool has_v1_inline = false;
         bool has_delta = false;   // some pages are DELTA_BINARY_PACKED: transcribed to PLAIN in the scratch buffer (pq_delta_to_plain)
         // list columns: the level sections of every data page (slot_start local to the chunk; pointers of pages decompressed here are
@@ -523,8 +527,10 @@ struct ParquetScanExec : Operator, FusedScanSource {
         const int64_t len = cm.total_compressed;
         const bool is_list = cs.shape == pq::SHAPE_LIST;
         const int max_def = is_list ? cs.max_def : el.repetition == 1 ? 1 : 0;
+        out.snappy_jobs = cm.codec == pq::CODEC_SNAPPY;
         const bool compressed = cm.codec != pq::CODEC_UNCOMPRESSED;
-        const bool dev_snappy = cm.codec == pq::CODEC_SNAPPY && gpu_snappy();
+        // SNAPPY, ZSTD and LZ4_RAW bodies are decompressed on the device (k_snappy.cu, k_zstd.cu) unless the host needs them
+        const bool dev_codec = (cm.codec == pq::CODEC_SNAPPY && gpu_snappy()) || cm.codec == pq::CODEC_ZSTD || cm.codec == pq::CODEC_LZ4_RAW;
         int64_t pos = 0, values_seen = 0, rows = is_list ? 0 : ct.row_start;   // (lists: rows counts values)
         int cur_dict = -1;
         while (pos < len && values_seen < cm.num_values) {
@@ -538,16 +544,20 @@ struct ParquetScanExec : Operator, FusedScanSource {
             int64_t unc_off = -1;
             int32_t lvl_bytes = h.type == pq::PAGE_DATA_V2 ? h.def_bytes + h.rep_bytes : 0;
             const bool page_compressed = compressed && !(h.type == pq::PAGE_DATA_V2 && !h.v2_compressed);
-            // Where the page body ends up: in place (uncompressed, or "stored" below), decompressed on the device (Snappy), or
-            // decompressed on the host (other codecs; and the one Snappy case whose levels the host must see: a PLAIN string
-            // page needs its non-null count to place its values, which a nullable v1 page only has inside its body).
+            // Where the page body ends up: in place (uncompressed, or "stored" below), decompressed on the device, or decompressed
+            // on the host (AURON_HOST_SNAPPY; and the pages whose body the host must see: a PLAIN string page needs its non-null count
+            // to place its values, which a nullable v1 page only has inside its body; delta strings are rewritten here).
             const bool delta_strings = is_string && (h.encoding == pq::ENC_DELTA_LENGTH_BYTE_ARRAY || h.encoding == pq::ENC_DELTA_BYTE_ARRAY);
             // (the levels of a v1 list page are inside its body: the host counts the page's values from them, so it decompresses the body)
-            const bool page_dev = dev_snappy && !(is_string && h.type == pq::PAGE_DATA && h.encoding == pq::ENC_PLAIN && max_def > 0) && !delta_strings &&
+            const bool page_dev = dev_codec && !(is_string && h.type == pq::PAGE_DATA && h.encoding == pq::ENC_PLAIN && max_def > 0) && !delta_strings &&
                                   !(is_list && h.type == pq::PAGE_DATA);
             bool on_device = false;
             int64_t gap = 0;   // stored v2 page with level sections: Snappy framing bytes between the levels and the values
-            if (page_compressed && page_dev) {
+            if (page_compressed) (page_dev ? out.pages_dev : out.pages_host)++;
+            if (page_compressed && page_dev && cm.codec != pq::CODEC_SNAPPY) {
+                AURON_CHECK(h.uncompressed_size >= lvl_bytes && h.compressed_size >= lvl_bytes, "corrupt parquet page sizes");
+                on_device = true;
+            } else if (page_compressed && page_dev) {
                 AURON_CHECK(h.uncompressed_size >= lvl_bytes && h.compressed_size >= lvl_bytes, "corrupt parquet page sizes");
                 // Incompressible pages (bit-packed dictionary indices of random keys) are one Snappy literal: preamble, literal
                 // tag, raw body.  The body is then already in HBM inside the chunk, a few bytes further on: no job, no copy.
@@ -578,7 +588,10 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 const uint8_t* body_d = payload_d + lvl_bytes;
                 const int64_t body_in = h.compressed_size - lvl_bytes, body_out = h.uncompressed_size - lvl_bytes;
                 int64_t head_in = 0, head_out = 0;
-                if (body_out > (64 << 10) && snappy_split(body_h, body_in, body_out, 4096, &head_in, &head_out, &pieces) &&
+                if (cm.codec != pq::CODEC_SNAPPY) {   // one job per page body: ZSTD frames or one LZ4 block
+                    out.jobs.push_back(PqDecompJob{body_d, (uint8_t*)(intptr_t)(unc_off + lvl_bytes), (int32_t)body_in, (int32_t)body_out,
+                                                   cm.codec == pq::CODEC_ZSTD ? PQ_JOB_ZSTD : PQ_JOB_LZ4, 0});
+                } else if (body_out > (64 << 10) && snappy_split(body_h, body_in, body_out, 4096, &head_in, &head_out, &pieces) &&
                     body_out - head_out >= (32 << 10) && !(v1_nullable && pieces.size() == 1)) {
                     int64_t dst = unc_off + lvl_bytes;
                     if (head_out > 0)   // kind 2: the preamble states the length of the whole body, the job ends after head_out bytes
@@ -1516,6 +1529,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
         std::unique_ptr<Prepared> ready;
         Buf status;            // page decompression status word (device)
         bool has_jobs = false;
+        std::vector<int8_t> job_codec;   // codec of every decompression job, for the error message
         cudaEvent_t dec0 = nullptr;
         bool tl = false;
     };
@@ -1581,8 +1595,8 @@ struct ParquetScanExec : Operator, FusedScanSource {
             Buf host_unc;   // chunks decompressed on the host: their payload, uploaded below
         };
         std::vector<Slot> slots(p.tasks.size());
-        int64_t unc_total = 0;
-        size_t n_jobs = 0;
+        int64_t unc_total = 0, pages_dev = 0, pages_host = 0;
+        size_t n_jobs = 0, n_other_jobs = 0;   // Snappy jobs first, then the ZSTD / LZ4_RAW chunks' jobs (pq_decompress)
         std::vector<size_t> npages(p.cols.size(), 0), ndicts(p.cols.size(), 0), nsecs(p.cols.size(), 0);
         for (size_t ti = 0; ti < p.tasks.size(); ti++) {
             ChunkTask& ct = p.tasks[ti];
@@ -1591,8 +1605,15 @@ struct ParquetScanExec : Operator, FusedScanSource {
             Slot& sl = slots[ti];
             sl.unc_off = unc_total;
             unc_total += (cp.gpu_unc_bytes + 255) & ~(int64_t)255;
-            sl.job_base = n_jobs;
-            n_jobs += cp.jobs.size();
+            if (cp.snappy_jobs) {
+                sl.job_base = n_jobs;
+                n_jobs += cp.jobs.size();
+            } else {
+                sl.job_base = n_other_jobs;   // rebased behind the Snappy jobs below
+                n_other_jobs += cp.jobs.size();
+            }
+            pages_dev += cp.pages_dev;
+            pages_host += cp.pages_host;
             sl.page_base = npages[ct.col];
             sl.dict_base = ndicts[ct.col];
             sl.sec_base = nsecs[ct.col];
@@ -1637,6 +1658,12 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 cs.n_vals += cp.n_vals;
             }
         }
+        for (size_t ti = 0; ti < p.tasks.size(); ti++)
+            if (!p.tasks[ti].out.snappy_jobs) slots[ti].job_base += n_jobs;
+        const size_t n_snappy_jobs = n_jobs;
+        n_jobs += n_other_jobs;
+        metrics.add("pages_decompressed_device", pages_dev);
+        metrics.add("pages_decompressed_host", pages_host);
         uint8_t* unc_scratch = nullptr;   // one scratch block for every device-decompressed page of the batch
         if (unc_total > 0) {
             p.unc_device = t.ctx.device;
@@ -1707,8 +1734,11 @@ struct ParquetScanExec : Operator, FusedScanSource {
         {
             Ctx& dc = (use_lanes && !decomp_jobs.empty()) ? lane(t, kLanes) : wc;
             if (&dc != &wc) chain(wc.stream, dc.stream);   // scratch allocated, chunk bytes uploaded
-            PqDecompOut dec = pq_decompress(dc, decomp_jobs);
+            PqDecompOut dec = pq_decompress(dc, decomp_jobs, n_snappy_jobs);
             sg.status = dec.status;
+            sg.job_codec.resize(decomp_jobs.size());
+            for (size_t j = 0; j < decomp_jobs.size(); j++)
+                sg.job_codec[j] = decomp_jobs[j].kind == PQ_JOB_ZSTD ? pq::CODEC_ZSTD : decomp_jobs[j].kind == PQ_JOB_LZ4 ? pq::CODEC_LZ4_RAW : pq::CODEC_SNAPPY;
             bool any_delta = false;
             for (auto& cs : p.cols) any_delta = any_delta || cs.has_delta;
             sg.has_jobs = !decomp_jobs.empty() || any_delta;
@@ -1730,7 +1760,14 @@ struct ParquetScanExec : Operator, FusedScanSource {
         if (!sg.has_jobs) return;
         int32_t st = 0;
         to_host(t.ctx, &st, sg.status->ptr, 4);
-        AURON_CHECK(st == 0, st >= 0x40000000 ? std::string("corrupt DELTA_BINARY_PACKED page in the parquet file") : "corrupt Snappy page in the parquet file (decompression job " + std::to_string(st - 1) + ")");
+        if (st != 0) fail(decomp_error(sg, st));
+    }
+    static std::string decomp_error(const Staged& sg, int32_t st) {
+        if (st >= 0x40000000) return "corrupt DELTA_BINARY_PACKED page in the parquet file";
+        const size_t j = (size_t)(st - 1);
+        const int codec = j < sg.job_codec.size() ? sg.job_codec[j] : pq::CODEC_SNAPPY;
+        const char* name = codec == pq::CODEC_ZSTD ? "ZSTD" : codec == pq::CODEC_LZ4_RAW ? "LZ4_RAW" : "Snappy";
+        return std::string("corrupt ") + name + " page in the parquet file (decompression job " + std::to_string(j) + ")";
     }
 
     BatchPtr next(Task& t) override {
@@ -1824,7 +1861,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
         if (f->sg.has_jobs) {
             int32_t st = 0;
             CUDA_OK(cudaMemcpy(&st, f->sg.status->ptr, 4, cudaMemcpyDeviceToHost));   // the batch is complete: plain copy, no stream involved
-            AURON_CHECK(st == 0, st >= 0x40000000 ? std::string("corrupt DELTA_BINARY_PACKED page in the parquet file") : "corrupt Snappy page in the parquet file (decompression job " + std::to_string(st - 1) + ")");
+            if (st != 0) fail(decomp_error(f->sg, st));
         }
     }
     void retire_fused(Task& t) {

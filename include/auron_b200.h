@@ -166,6 +166,10 @@ int auron_b200_float_to_text(int32_t bits, uint64_t value, char* out);
  * or float64 (bits 64) bit pattern to *value and returns 1, returns 0 where the cast gives NULL, -1 for a bad argument.
  * Host only: usable without a GPU. */
 int auron_b200_text_to_float(int32_t bits, const uint8_t* text, int64_t len, uint64_t* value);
+/* Decompress the ZSTD data in[0, in_len) (Zstandard and skippable frames back to back, a Parquet ZSTD page body) into out[0, out_len)
+ * with the decoder the Parquet scan runs on the device.  Returns the bytes written, or -1 (auron_b200_last_error) when the data are
+ * malformed or decode to more than out_len bytes.  Host only: usable without a GPU. */
+int64_t auron_b200_zstd_decompress(const uint8_t* in, int64_t in_len, uint8_t* out, int64_t out_len);
 /* What the engine's Parquet metadata reader sees in the local file `path`, as JSON: footer (schema elements, row groups, column
  * chunks with codec / sizes / offsets / statistics as hex) plus, per chunk, the walk of its page headers (page counts, value
  * counts, encodings; SNAPPY bodies are run through the engine's block decoder).  The reference reads the same structures with

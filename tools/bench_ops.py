@@ -3,7 +3,7 @@ time per launch site from the library's CUDA-event timers (AURON_PROFILE=1).  Th
 north star asks for next to the config-2 bench line; they are not bench.py lines.
 
     python tools/bench_ops.py [join] [sort] [shuffle] [agg_lowcard] [strings] [filter_project] [scalar] [casts] [window] [generate]
-                              [parquet_list]
+                              [parquet_list] [parquet_zstd]
 
   join     cfg 3: store_sales (N rows: ss_sold_date_sk int32, ss_item_sk int32, ss_quantity int32) JOIN date_dim (73,049 rows:
            d_date_sk int32, d_year int32) on the date key, inner, build = date_dim
@@ -35,6 +35,11 @@ north star asks for next to the config-2 bench line; they are not bench.py lines
            then the config-2 fused leg (SNAPPY Parquet of N rows item / qty / date int32 -> Filter -> partial SUM / COUNT by item,
            best of 5 passes) and the Filter -> Project leg three times each, each time followed by the same leg of the built checkout
            at $OPS_PARENT when that is set
+  parquet_zstd  the config-2 file (N rows item / qty / date int32, dictionary pages) written with ZSTD level 1, ZSTD level 3 and
+           LZ4_RAW, its image resident in HBM (put_device_file) -> Filter -> partial SUM / COUNT by item.  Reports the device time of
+           the page decompression kernels (pq_zstd, lz4_decompress) with compressed and uncompressed GB/s (the chunks' compressed and
+           uncompressed sizes from the footer), then the whole pass (best of 5) three times, each time followed by the same pass of
+           the built checkout at $OPS_PARENT when that is set
 """
 import os
 import sys
@@ -524,3 +529,72 @@ print(f"fused_ms {1000 * best:.1f} groups {rows} fused_batches {fused}")
                                  cwd=parent, env=dict(os.environ, OPS_ROWS=str(N))).stdout
             ms = re.search(r"expr_vm\s+([0-9.]+) ms", out)
             print(f"== Filter -> Project, parent tree, pass {k + 1}: expr_vm {ms.group(1) if ms else '?'} ms")
+
+if "parquet_zstd" in which:
+    import subprocess
+    import tempfile
+
+    import pyarrow.parquet as pq
+
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    print(f"== parquet_zstd leg on: {gpu}")
+    tab = pa.table({"item": pa.array(rng.integers(1, 204001, N).astype(np.int32)),
+                    "qty": pa.array(rng.integers(1, 101, N).astype(np.int32), mask=rng.random(N) < 0.03),
+                    "date": pa.array(rng.integers(2450816, 2452642, N).astype(np.int32), mask=rng.random(N) < 0.04)})
+    leg = """
+import os, sys, time
+sys.path.insert(0, os.getcwd())
+import pyarrow as pa
+from auron_b200 import proto as P
+from auron_b200 import runtime
+path = sys.argv[1]
+data = open(path, "rb").read()
+runtime.put_device_file("hbm://cfg2", data)
+I32, I64 = pa.int32(), pa.int64()
+sch = pa.schema([("item", I32), ("qty", I32), ("date", I32)])
+flt = P.filter_(P.parquet_scan(sch, [("hbm://cfg2", len(data))], [0, 1, 2]),
+                [P.binary("GtEq", P.col("date"), P.lit(2451000, I32)), P.binary("Lt", P.col("date"), P.lit(2452000, I32))])
+plan = P.agg(flt, [P.try_cast(P.col("item"), I64)], ["item"], [P.agg_expr("SUM", [P.col("qty")], I64), P.agg_expr("COUNT", [P.col("qty")], I64)],
+             ["s", "c"], ["PARTIAL", "PARTIAL"])
+best, fused, total = None, 0, 0
+for _ in range(5):
+    t0 = time.perf_counter()
+    with runtime.Task(P.task_definition(plan)) as task:
+        rows, tot = 0, 0
+        for b in task:
+            rows += b.num_rows
+            tot += sum(x for x in b.column(2).to_pylist() if x)
+        fused = sum(v for _, _, n, v in task.metrics() if n == "fused_batches")
+    dt = time.perf_counter() - t0
+    best = dt if best is None else min(best, dt)
+print(f"pass_ms {1000 * best:.1f} groups {rows} count {tot} fused_batches {fused}")
+"""
+    here = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    parent = os.environ.get("OPS_PARENT")
+    with tempfile.TemporaryDirectory() as d:
+        for codec, level in (("ZSTD", 1), ("ZSTD", 3), ("LZ4_RAW", None)):
+            path = os.path.join(d, f"cfg2_{codec}_{level}.parquet")
+            pq.write_table(tab, path, compression=codec, row_group_size=8 << 20, **({"compression_level": level} if level else {}))
+            md = pq.ParquetFile(path).metadata
+            comp = sum(md.row_group(g).column(c).total_compressed_size for g in range(md.num_row_groups) for c in range(md.num_columns))
+            unc = sum(md.row_group(g).column(c).total_uncompressed_size for g in range(md.num_row_groups) for c in range(md.num_columns))
+            name = f"{codec}" + (f" level {level}" if level else "")
+            data = open(path, "rb").read()
+            runtime.put_device_file("hbm://zs", data)
+            sch = tab.schema
+            flt = P.filter_(P.parquet_scan(sch, [("hbm://zs", len(data))], [0, 1, 2]),
+                            [P.binary("GtEq", P.col("date"), P.lit(2451000, pa.int32())), P.binary("Lt", P.col("date"), P.lit(2452000, pa.int32()))])
+            plan = P.agg(flt, [P.try_cast(P.col("item"), pa.int64())], ["item"],
+                         [P.agg_expr("SUM", [P.col("qty")], pa.int64()), P.agg_expr("COUNT", [P.col("qty")], pa.int64())], ["s", "c"], ["PARTIAL", "PARTIAL"])
+            kern = run(plan, f"config-2 {name} image in HBM ({comp >> 20} MiB compressed, {unc >> 20} MiB uncompressed) -> Filter -> SUM / COUNT by item over {N} rows",
+                       N, steps=3)
+            for site in ("pq_zstd", "lz4_decompress"):
+                if kern.get(site):
+                    sec = kern[site] * 1e-6
+                    print(f"     {site}: {comp / sec / 1e9:.1f} GB/s compressed in, {unc / sec / 1e9:.1f} GB/s uncompressed out, "
+                          f"{(comp + unc) / sec / 1e9:.1f} GB/s algorithmic")
+            runtime.drop_device_file("hbm://zs")
+            for k in range(3):
+                for label, root in [("this tree", here)] + ([("parent tree", parent)] if parent else []):
+                    out = subprocess.run([sys.executable, "-c", leg, path], capture_output=True, text=True, cwd=root)
+                    print(f"== config-2 {name} pass over {N} rows, {label}, round {k + 1}: {out.stdout.strip() or out.stderr.strip()[-300:]}")
