@@ -14,7 +14,8 @@
 //               are decoded in place;
 //               delta-encoded string pages are rewritten as PLAIN, Hive partition columns become constant columns, row groups
 //               that the pruning predicates exclude by their statistics are skipped at plan time
-//   4. decode : k_parquet.cu, one scout launch for all columns + one decode launch per column -- or, when the plan above is
+//   4. decode : k_parquet.cu, one scout launch for all flat columns + one decode launch per column (a list column scouts its
+//               element values on its own and builds its layout with k_parquet_levels.cu) -- or, when the plan above is
 //               Filter -> HashAggregate of the supported shape, next_fused(): the batch goes through k_fused.cu instead and no
 //               column is materialised (three batches in flight on their own stream pairs, see next_fused)
 #include <dlfcn.h>
@@ -425,7 +426,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
         int64_t value_table_size = 0;
         std::vector<Buf> keep;
         bool has_v1_inline = false;   // some v1 pages still need their level / value sections split on the device
-        bool needs_decomp = false;    // some pages of this column are produced by the batch's decompression launch
         bool has_delta = false;
         // bounds of the non-null values from the column-chunk statistics of every chunk in the batch (INT32 / INT64)
         bool stat_ok = true;
@@ -438,38 +438,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
         std::vector<PqLevelPage> levels;
         int64_t n_slots = 0, n_vals = 0;
     };
-
-    // host-side count of non-null values of a v1 page (needed only for PLAIN string pages)
-    static int32_t count_non_null_v1(const uint8_t* payload, int max_def, int32_t num_values) {
-        if (max_def == 0) return num_values;
-        uint32_t dl;
-        memcpy(&dl, payload, 4);
-        const uint8_t* p = payload + 4;
-        const uint8_t* end = p + dl;
-        int32_t seen = 0, nn = 0;
-        while (p < end && seen < num_values) {
-            uint32_t h = 0;
-            int shift = 0;
-            while (p < end) {
-                uint8_t b = *p++;
-                h |= (uint32_t)(b & 0x7f) << shift;
-                if (!(b & 0x80)) break;
-                shift += 7;
-            }
-            if (h & 1) {
-                int cnt = (int)(h >> 1) * 8;
-                for (int i = 0; i < cnt && seen < num_values; i++, seen++) nn += (p[i >> 3] >> (i & 7)) & 1;
-                p += h >> 1;
-            } else {
-                int cnt = (int)(h >> 1);
-                int v = *p++ & 1;
-                int take = std::min(cnt, num_values - seen);
-                nn += v * take;
-                seen += take;
-            }
-        }
-        return nn;
-    }
 
     // `p[0, n)` is a Snappy block of `unc` bytes made of exactly one literal element: returns the offset of the literal's
     // bytes (> 0), else 0
@@ -497,17 +465,8 @@ struct ParquetScanExec : Operator, FusedScanSource {
         }
         return (len == unc && i + len == n) ? i : 0;
     }
-    // `p[0, n)` is a Snappy block of `unc` bytes made only of literals (incompressible data: one literal per 64 KB fragment of
-    // the compressor): fills their (offset in p, length) and returns true; at most `max_pieces`
-    using LitPiece = pq::LitPiece;
-    // (the tag walk of a Snappy block and the host decoders of the delta string encodings live in parquet_meta.cc, where
-    // auron_b200_parquet_describe exercises them on the CPU)
-    static bool snappy_split(const uint8_t* p, int64_t n, int64_t unc, int max_tokens, int64_t* head_in, int64_t* head_out, std::vector<LitPiece>* pieces) {
-        return pq::snappy_split(p, n, unc, max_tokens, head_in, head_out, pieces);
-    }
-    static std::vector<uint8_t> delta_strings_to_plain(const uint8_t* p, size_t n, bool front_coded, int32_t* n_values, size_t max_values) {
-        return pq::delta_strings_to_plain(p, n, front_coded, n_values, max_values);
-    }
+    // (the tag walk of a Snappy block, pq::snappy_split, and the host decoders of the delta string encodings and of level streams live
+    // in parquet_meta.cc, where auron_b200_parquet_describe exercises them on the CPU)
     static bool gpu_snappy() {
         return getenv("AURON_HOST_SNAPPY") == nullptr;   // AURON_HOST_SNAPPY=1: decompress on the host cores instead
     }
@@ -582,7 +541,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 // become independent stored-copy jobs of <= 16 KB, the elements before them a short Snappy job of their own.
                 // Not split: a body whose tail is ONE literal in a nullable v1 page (the decoder leaves that one in place), and
                 // bodies of many elements (compressible data: the walk stops after 4096 tags).
-                std::vector<LitPiece> pieces;
+                std::vector<pq::LitPiece> pieces;
                 const bool v1_nullable = h.type == pq::PAGE_DATA && max_def > 0;
                 const uint8_t* body_h = payload_h + lvl_bytes;
                 const uint8_t* body_d = payload_d + lvl_bytes;
@@ -591,7 +550,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 if (cm.codec != pq::CODEC_SNAPPY) {   // one job per page body: ZSTD frames or one LZ4 block
                     out.jobs.push_back(PqDecompJob{body_d, (uint8_t*)(intptr_t)(unc_off + lvl_bytes), (int32_t)body_in, (int32_t)body_out,
                                                    cm.codec == pq::CODEC_ZSTD ? PQ_JOB_ZSTD : PQ_JOB_LZ4, 0});
-                } else if (body_out > (64 << 10) && snappy_split(body_h, body_in, body_out, 4096, &head_in, &head_out, &pieces) &&
+                } else if (body_out > (64 << 10) && pq::snappy_split(body_h, body_in, body_out, 4096, &head_in, &head_out, &pieces) &&
                     body_out - head_out >= (32 << 10) && !(v1_nullable && pieces.size() == 1)) {
                     int64_t dst = unc_off + lvl_bytes;
                     if (head_out > 0)   // kind 2: the preamble states the length of the whole body, the job ends after head_out bytes
@@ -711,7 +670,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
             if (delta_strings) {   // (never on_device: the body is on the host, in the file image or in out.unc)
                 const std::vector<uint8_t> head(hp(0), hp(0) + o);
                 int32_t nn = 0;
-                const std::vector<uint8_t> plain = delta_strings_to_plain(hp(o + gap), (size_t)(total - o - gap), h.encoding == pq::ENC_DELTA_BYTE_ARRAY, &nn, (size_t)h.num_values);
+                const std::vector<uint8_t> plain = pq::delta_strings_to_plain(hp(o + gap), (size_t)(total - o - gap), h.encoding == pq::ENC_DELTA_BYTE_ARRAY, &nn, (size_t)h.num_values);
                 AURON_CHECK(list_nn < 0 || nn == list_nn, "corrupt parquet list page: its values do not match its levels (column " + cs.path + ")");
                 unc_off = (int64_t)out.unc.size();
                 out.unc.resize(out.unc.size() + head.size() + plain.size() + 8);
@@ -733,8 +692,10 @@ struct ParquetScanExec : Operator, FusedScanSource {
             }
             size_t sec_idx = SIZE_MAX;
             if (is_string && pg.encoding == pq::ENC_PLAIN) {
-                // PLAIN string pages need their exact non-null count: v2 gives it, v1 requires the def levels
-                int32_t nn = delta_nn >= 0 ? delta_nn : list_nn >= 0 ? list_nn : h.type == pq::PAGE_DATA_V2 ? h.num_values - h.num_nulls : count_non_null_v1(hp(0), max_def, h.num_values);
+                // PLAIN string pages need their exact non-null count: v2 gives it, v1 requires the def levels (whose section, behind the
+                // length word, lies inside the page: o <= total above)
+                int32_t nn = delta_nn >= 0 ? delta_nn : list_nn >= 0 ? list_nn : h.type == pq::PAGE_DATA_V2 ? h.num_values - h.num_nulls : max_def == 0 ? h.num_values
+                           : (int32_t)pq::hybrid_count(hp(4), (size_t)pg.def_len, 1, h.num_values, 1);
                 pg.plain_value_base = (int32_t)out.value_table_size;
                 sec_idx = out.secs.size();
                 out.secs.push_back({base_d ? pg.val_ptr : nullptr, pg.val_len, nn, (int32_t)out.value_table_size});
@@ -915,17 +876,43 @@ struct ParquetScanExec : Operator, FusedScanSource {
     const PqDecompResult* decomp_results = nullptr;   // results of the current batch's decompression launch (device)
     uint8_t* unc_scratch_ptr = nullptr;               // the current batch's scratch buffer and status word (device)
     int32_t* status_ptr = nullptr;
-    cudaEvent_t decomp_done = nullptr;                // recorded on the decompression lane (nullptr: nothing to wait for)
-    // Side streams ("lanes"): the decompress -> scout -> decode chains of a batch's columns are independent, and each of
-    // these kernels leaves most of the GPU idle on its own (latency-bound header walks, L1-bound gathers), so the chains
-    // run concurrently -- column c on lane c % kLanes, page decompression on its own lane.  Output buffers are allocated on
-    // the task stream (their lifetime follows the batch); lanes only own temporaries.
-    // The chains compete for the same L1 / LSU pipes and for HBM, so overlapping them conserves the total; the mode stays
-    // opt-in (AURON_SCAN_LANES=1).
-    static constexpr int kLanes = 3;
+    // The device copies of a column's page and dictionary descriptors, fixed up for the decoders on `ctx` in this order: the level /
+    // value sections of v1 pages decompressed on the device (pq_fix_v1_pages), then the PLAIN transcription of DELTA_BINARY_PACKED
+    // pages into the batch's scratch buffer (pq_delta_to_plain)
+    struct ColDescriptors {
+        Buf pages, dicts;
+    };
+    ColDescriptors upload_descriptors(Ctx& ctx, const ColState& cs) const {
+        ColDescriptors d;
+        d.pages = to_device(ctx, cs.pages.empty() ? (const void*)"" : (const void*)cs.pages.data(), cs.pages.size() * sizeof(PqPage));
+        d.dicts = to_device(ctx, cs.dicts.empty() ? (const void*)"" : (const void*)cs.dicts.data(), cs.dicts.size() * sizeof(PqDict));
+        if (cs.has_v1_inline) pq_fix_v1_pages(ctx, P<PqPage>(d.pages), (int)cs.pages.size(), decomp_results);
+        if (cs.has_delta) pq_delta_to_plain(ctx, P<PqPage>(d.pages), (int)cs.pages.size(), unc_scratch_ptr, cs.el.type == pq::PT_INT32 ? 4 : 8, status_ptr);
+        return d;
+    }
+    // decode arguments of a column whose values are read as type `t` (a list column: its element type); the caller sets the mode
+    // and the outputs
+    static PqColumnArgs column_args(const ColState& cs, const ColDescriptors& d, const DType& t, int max_def) {
+        PqColumnArgs a;
+        memset(&a, 0, sizeof(a));
+        a.pages = P<PqPage>(d.pages);
+        a.dicts = P<PqDict>(d.dicts);
+        a.n_pages = (int)cs.pages.size();
+        a.phys_type = cs.el.type;
+        a.type_length = cs.el.type_length;
+        a.phys_width = phys_width(cs.el.type, cs.el.type_length);
+        a.out_type = t.id;
+        a.out_width = t.width();
+        a.out_unit = t.unit;
+        a.conv = cs.cv.kind;
+        a.conv_mul = cs.cv.mul;
+        a.conv_mul_hi = cs.cv.mul_hi;
+        a.max_def = max_def;
+        return a;
+    }
+    // side streams ("lanes") of the fused path, see next_fused
     std::vector<std::unique_ptr<Ctx>> lanes;
     std::vector<int> lane_priority;
-    bool use_lanes = getenv("AURON_SCAN_LANES") != nullptr;
     // Lane contexts (a stream + its staged-upload arena) outlive the scan that used them: every task is a new ParquetScanExec, and six
     // stream creations / destructions per task are host time inside a step of a few milliseconds; idle lanes wait in a process-wide pool instead
     // (which also keeps the stream-ordered allocator's per-stream caches warm).
@@ -1003,27 +990,10 @@ struct ParquetScanExec : Operator, FusedScanSource {
     // the level pass (k_parquet_levels.cu) gives the offsets, the list validity and each element's value, one gather places the values.
     ColumnPtr build_list_column(Task& t, ColState& cs, const Field& fld, int64_t n_rows) {
         const DType& et = *fld.type.elem;
-        const pq::SchemaElement& el = cs.el;
         const int64_t nv = cs.n_vals;
         AURON_CHECK(nv <= cs.n_slots, "corrupt parquet list column " + cs.path + ": more values than level slots");
-        Buf dpages = to_device(t.ctx, cs.pages.empty() ? (const void*)"" : (const void*)cs.pages.data(), cs.pages.size() * sizeof(PqPage));
-        Buf ddicts = to_device(t.ctx, cs.dicts.empty() ? (const void*)"" : (const void*)cs.dicts.data(), cs.dicts.size() * sizeof(PqDict));
-        if (cs.has_delta) pq_delta_to_plain(t.ctx, P<PqPage>(dpages), (int)cs.pages.size(), unc_scratch_ptr, el.type == pq::PT_INT32 ? 4 : 8, status_ptr);
-        PqColumnArgs a;
-        memset(&a, 0, sizeof(a));
-        a.pages = P<PqPage>(dpages);
-        a.dicts = P<PqDict>(ddicts);
-        a.n_pages = (int)cs.pages.size();
-        a.phys_type = el.type;
-        a.type_length = el.type_length;
-        a.phys_width = phys_width(el.type, el.type_length);
-        a.out_type = et.id;
-        a.out_width = et.width();
-        a.out_unit = et.unit;
-        a.conv = cs.cv.kind;
-        a.conv_mul = cs.cv.mul;
-        a.conv_mul_hi = cs.cv.mul_hi;
-        a.max_def = 0;   // the values of a list page have no gaps
+        const ColDescriptors d = upload_descriptors(t.ctx, cs);
+        PqColumnArgs a = column_args(cs, d, et, 0);   // (the values of a list page have no gaps)
         ColumnPtr vals;   // fixed-width: the values; strings: the value table, gathered once through str_idx below
         Buf str_idx;      // strings: value -> entry of the value table
         if (cs.is_string) {
@@ -1078,18 +1048,17 @@ struct ParquetScanExec : Operator, FusedScanSource {
         AURON_CHECK(n_rows < (int64_t)INT32_MAX, "parquet batch too large");
         auto out = std::make_shared<Batch>();
         out->num_rows = n_rows;
-        // One scout launch for all columns of the batch (a column alone is a few thousand page-warps, too few for 132 SMs):
+        // One scout launch for all flat columns of the batch (a column alone is a few thousand page-warps, too few for 132 SMs):
         // the per-column work is prepared in the loop, scouted together, then decoded column by column.
-        // AURON_SCAN_SCOUT_PER_COLUMN=1 keeps one scout launch per column; the lane mode does too.
         struct Pending {
             size_t out_pos;
             PqPrepared pr;
             ColumnPtr table;   // strings: value table to gather from after the index decode
-            Buf idx, keep_pages, keep_dicts;
+            Buf idx;
+            ColDescriptors descr;
             bool nullable;
         };
         std::vector<Pending> pending;
-        const bool batch_scout = !use_lanes && !getenv("AURON_SCAN_SCOUT_PER_COLUMN");
         for (size_t ci = 0; ci < projection.size(); ci++) {
             const Field& fld = proj_field(projection[ci]);
             ColState& cs = cols[ci];
@@ -1129,74 +1098,39 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 continue;
             }
             if (cs.shape == pq::SHAPE_LIST) {
-                if (cs.needs_decomp && decomp_done) CUDA_OK(cudaStreamWaitEvent(t.ctx.stream, decomp_done, 0));
                 out->cols.push_back(build_list_column(t, cs, fld, n_rows));
                 continue;
             }
-            const pq::SchemaElement& el = cs.el;
-            const bool is_string = cs.is_string;
-            const int max_def = el.repetition == 1 ? 1 : 0;
-            PqColumnArgs a;
-            memset(&a, 0, sizeof(a));
-            // fixed-width columns decode on a lane; strings (value table + take) stay on the task stream
-            Ctx& wc = (use_lanes && !is_string) ? lane(t, (int)(ci % kLanes)) : t.ctx;
-            Buf validity;
+            const int max_def = cs.el.repetition == 1 ? 1 : 0;
             ColumnPtr col;
-            if (max_def > 0 || cs.cv.kind == PQ_CV_TS_MUL) validity = dalloc_zero(t.ctx, bitmap_alloc_bytes(n_rows));   // (overflowing products are NULL)
-            if (!is_string) {
+            Buf validity;
+            if (!cs.is_string) {
+                if (max_def > 0 || cs.cv.kind == PQ_CV_TS_MUL) validity = dalloc_zero(t.ctx, bitmap_alloc_bytes(n_rows));   // (overflowing products are NULL)
                 col = std::make_shared<Column>();
                 col->type = fld.type;
                 col->len = n_rows;
                 if (fld.type.id == T_BOOL) col->data = dalloc_zero(t.ctx, bitmap_alloc_bytes(n_rows));
                 else col->data = dalloc(t.ctx, (size_t)n_rows * fld.type.width());
             }
-            if (&wc != &t.ctx) {
-                chain(t.ctx.stream, wc.stream);   // outputs allocated (and zeroed), chunk bytes uploaded
-                if (cs.needs_decomp && decomp_done) CUDA_OK(cudaStreamWaitEvent(wc.stream, decomp_done, 0));
-            } else if (cs.needs_decomp && decomp_done) {
-                CUDA_OK(cudaStreamWaitEvent(t.ctx.stream, decomp_done, 0));
-            }
-            Buf dpages = to_device(wc, cs.pages.data(), cs.pages.size() * sizeof(PqPage));
-            Buf ddicts = to_device(wc, cs.dicts.empty() ? (const void*)"" : (const void*)cs.dicts.data(), cs.dicts.size() * sizeof(PqDict));
-            if (cs.has_v1_inline) pq_fix_v1_pages(wc, P<PqPage>(dpages), (int)cs.pages.size(), decomp_results);
-            if (cs.has_delta) pq_delta_to_plain(wc, P<PqPage>(dpages), (int)cs.pages.size(), unc_scratch_ptr, el.type == pq::PT_INT32 ? 4 : 8, status_ptr);
-            a.pages = P<PqPage>(dpages);
-            a.dicts = P<PqDict>(ddicts);
-            a.n_pages = (int)cs.pages.size();
-            a.phys_type = el.type;
-            a.type_length = el.type_length;
-            a.phys_width = phys_width(el.type, el.type_length);
-            a.out_type = fld.type.id;
-            a.out_width = fld.type.width();
-            a.out_unit = fld.type.unit;
-            a.conv = cs.cv.kind;
-            a.conv_mul = cs.cv.mul;
-            a.conv_mul_hi = cs.cv.mul_hi;
-            a.max_def = max_def;
-            a.out_valid = P<uint32_t>(validity);
-            if (is_string) {
+            const ColDescriptors d = upload_descriptors(t.ctx, cs);
+            PqColumnArgs a = column_args(cs, d, fld.type, max_def);
+            if (cs.is_string) {
                 ColumnPtr table = pq_build_value_table(t.ctx, cs.secs, cs.value_table_size, fld.type);
                 Buf idx = dalloc(t.ctx, (size_t)std::max<int64_t>(n_rows, 1) * 4);
                 a.mode = PQ_MODE_INDEX;
                 a.out_idx = P<int32_t>(idx);
-                a.out_valid = nullptr;
-                if (batch_scout) {
-                    pending.push_back(Pending{out->cols.size(), pq_prepare(t.ctx, a, cs.pages), table, idx, dpages, ddicts, max_def > 0});
-                } else {
-                    pq_decode_pages(t.ctx, a, cs.pages);
-                    col = take(t.ctx, *table, P<int32_t>(idx), n_rows, max_def > 0);
-                }
+                pending.push_back(Pending{out->cols.size(), pq_prepare(t.ctx, a, cs.pages), table, idx, d, max_def > 0});   // (col: the take below)
             } else {
-                a.out = col->data->ptr;
                 a.mode = PQ_MODE_VALUES;
-                if (batch_scout) pending.push_back(Pending{out->cols.size(), pq_prepare(t.ctx, a, cs.pages), nullptr, nullptr, dpages, ddicts, false});
-                else pq_decode_pages(wc, a, cs.pages);
+                a.out = col->data->ptr;
+                a.out_valid = P<uint32_t>(validity);
+                pending.push_back(Pending{out->cols.size(), pq_prepare(t.ctx, a, cs.pages), nullptr, nullptr, d, false});
                 if (validity) {
                     col->validity = validity;
                     col->null_count = -1;
                 }
                 const TypeId ot = fld.type.id;
-                if (cs.stat_ok && cs.stat_min <= cs.stat_max && (ot == T_INT32 || ot == T_INT64 || ot == T_DATE32) && !getenv("AURON_SCAN_NO_STATS")) {
+                if (cs.stat_ok && cs.stat_min <= cs.stat_max && (ot == T_INT32 || ot == T_INT64 || ot == T_DATE32)) {
                     col->has_range = true;
                     col->range_min = cs.stat_min;
                     col->range_max = cs.stat_max;
@@ -1242,22 +1176,12 @@ struct ParquetScanExec : Operator, FusedScanSource {
     };
     cudaStream_t copy_stream = nullptr;
     int prefetch_depth = 3;
-    int64_t batches_planned = 0;
-    int64_t ramp_rows = getenv("AURON_SCAN_RAMP_ROWS") ? atoll(getenv("AURON_SCAN_RAMP_ROWS")) : 0;
     std::thread producer;
     std::mutex qmu;
     std::condition_variable qcv;
     std::deque<std::unique_ptr<Prepared>> ready_q;
     bool producer_started = false, producer_done = false, stop_producer = false;
     std::string producer_err;
-    // AURON_SCAN_TIMELINE=1 (with AURON_PROFILE=1): device-side timeline of every batch, printed when the scan ends
-    struct TimelineRow {
-        float copy0, copy1, dec0, dec1;
-        int64_t rows;
-    };
-    std::vector<TimelineRow> timeline;
-    cudaEvent_t tl_base = nullptr;
-    bool want_timeline = getenv("AURON_SCAN_TIMELINE") != nullptr;
 
     void release(Prepared& p) {
         if (p.pinned) pinned_pool().put(p.pinned, p.pinned_cap);
@@ -1293,9 +1217,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
             }
             const auto& rg = cur->meta.row_groups[cur->row_groups[rg_pos]];
             std::string sig = signature(*cur);
-            // ramp-up: the first batch is small so that the GPU starts while the remaining page headers are still being parsed
-            const int64_t limit = batches_planned == 0 && ramp_rows > 0 ? std::min(ramp_rows, t.ctx.gpu_chunk_rows) : t.ctx.gpu_chunk_rows;
-            if (started && (sig != batch_sig || p.rows + rg.num_rows > limit)) break;
+            if (started && (sig != batch_sig || p.rows + rg.num_rows > t.ctx.gpu_chunk_rows)) break;
             if (!started) {
                 started = true;
                 batch_sig = sig;
@@ -1333,7 +1255,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
             rg_pos++;
         }
         if (!started) return nullptr;
-        batches_planned++;
         // chunk placement: HBM-resident images in place, host files into one pinned staging buffer + one device buffer
         for (auto& ct : p.tasks) {
             int64_t start = ct.cm->start_offset(), len = ct.cm->total_compressed;
@@ -1480,7 +1401,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
         for (auto& f : inflight) {   // fused batches still running: their landing buffers go back only once the kernels are done
             cudaEventSynchronize(f->done);
             cudaEventDestroy(f->done);
-            if (f->sg.dec0) cudaEventDestroy(f->sg.dec0);
             release(*f->sg.ready);
         }
         inflight.clear();
@@ -1530,8 +1450,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
         Buf status;            // page decompression status word (device)
         bool has_jobs = false;
         std::vector<int8_t> job_codec;   // codec of every decompression job, for the error message
-        cudaEvent_t dec0 = nullptr;
-        bool tl = false;
     };
     // nullptr ready = end of the scan
     // `wc`: the context (stream) the batch's device work is queued on -- the task's own, or one of the two lanes the fused path alternates between
@@ -1548,20 +1466,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
                 metrics.add("row_groups_pruned", row_groups_pruned);
                 row_groups_pruned = 0;
             }
-            if (want_timeline && !timeline.empty()) {
-                for (size_t i = 0; i < timeline.size(); i++)
-                    fprintf(stderr, "[scan timeline] batch %zu rows=%lld  copy %.2f..%.2f ms  decode %.2f..%.2f ms\n", i, (long long)timeline[i].rows,
-                            timeline[i].copy0, timeline[i].copy1, timeline[i].dec0, timeline[i].dec1);
-                timeline.clear();
-            }
             return sg;
-        }
-        const bool tl = want_timeline && t.ctx.profile;
-        sg.tl = tl;
-        cudaEvent_t dec0 = nullptr;
-        if (tl && !tl_base) {
-            CUDA_OK(cudaEventCreate(&tl_base));
-            CUDA_OK(cudaEventRecord(tl_base, t.ctx.stream));
         }
         struct Guard {   // an exception below must not leak the landing buffers
             ParquetScanExec* op;
@@ -1576,10 +1481,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
         if (ready->dev_bytes) {
             metrics.add("h2d_bytes", ready->dev_bytes);
             CUDA_OK(cudaStreamWaitEvent(wc.stream, ready->copied, 0));
-        }
-        if (tl) {
-            CUDA_OK(cudaEventCreate(&dec0));
-            CUDA_OK(cudaEventRecord(dec0, wc.stream));
         }
         Prepared& p = *ready;
         // ordered merge, rebasing dictionary ids / value-table positions; compressed chunks upload their payloads first
@@ -1625,7 +1526,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
             if (cp.gpu_unc_bytes > 0) {
                 cs.has_v1_inline = cs.has_v1_inline || cp.has_v1_inline;
                 cs.has_delta = cs.has_delta || cp.has_delta;
-                cs.needs_decomp = true;
             }
             {   // statistics -> bounds of the converted values
                 const pq::Statistics& st = ct.cm->stats;
@@ -1731,27 +1631,18 @@ struct ParquetScanExec : Operator, FusedScanSource {
             }
         });
         delete tmerge;
-        {
-            Ctx& dc = (use_lanes && !decomp_jobs.empty()) ? lane(t, kLanes) : wc;
-            if (&dc != &wc) chain(wc.stream, dc.stream);   // scratch allocated, chunk bytes uploaded
-            PqDecompOut dec = pq_decompress(dc, decomp_jobs, n_snappy_jobs);
-            sg.status = dec.status;
-            sg.job_codec.resize(decomp_jobs.size());
-            for (size_t j = 0; j < decomp_jobs.size(); j++)
-                sg.job_codec[j] = decomp_jobs[j].kind == PQ_JOB_ZSTD ? pq::CODEC_ZSTD : decomp_jobs[j].kind == PQ_JOB_LZ4 ? pq::CODEC_LZ4_RAW : pq::CODEC_SNAPPY;
-            bool any_delta = false;
-            for (auto& cs : p.cols) any_delta = any_delta || cs.has_delta;
-            sg.has_jobs = !decomp_jobs.empty() || any_delta;
-            unc_scratch_ptr = unc_scratch;
-            status_ptr = P<int32_t>(dec.status);
-            decomp_results_buf = dec.results;
-            decomp_results = P<PqDecompResult>(dec.results);
-            if (&dc != &wc) {
-                CUDA_OK(cudaEventCreateWithFlags(&decomp_done, cudaEventDisableTiming));
-                CUDA_OK(cudaEventRecord(decomp_done, dc.stream));
-            }
-        }
-        sg.dec0 = dec0;
+        PqDecompOut dec = pq_decompress(wc, decomp_jobs, n_snappy_jobs);
+        sg.status = dec.status;
+        sg.job_codec.resize(decomp_jobs.size());
+        for (size_t j = 0; j < decomp_jobs.size(); j++)
+            sg.job_codec[j] = decomp_jobs[j].kind == PQ_JOB_ZSTD ? pq::CODEC_ZSTD : decomp_jobs[j].kind == PQ_JOB_LZ4 ? pq::CODEC_LZ4_RAW : pq::CODEC_SNAPPY;
+        bool any_delta = false;
+        for (auto& cs : p.cols) any_delta = any_delta || cs.has_delta;
+        sg.has_jobs = !decomp_jobs.empty() || any_delta;
+        unc_scratch_ptr = unc_scratch;
+        status_ptr = P<int32_t>(dec.status);
+        decomp_results_buf = dec.results;
+        decomp_results = P<PqDecompResult>(dec.results);
         sg.ready = std::move(ready);
         return sg;
     }
@@ -1791,8 +1682,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
                     cudaStreamSynchronize(st);
                 }
                 op->release(*p);
-                if (op->decomp_done) cudaEventDestroy(op->decomp_done);
-                op->decomp_done = nullptr;
                 op->decomp_results = nullptr;
                 op->decomp_results_buf.reset();
             }
@@ -1808,23 +1697,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
             CUDA_OK(cudaEventSynchronize(p.copied));
             CUDA_OK(cudaEventElapsedTime(&ms, p.copy_begin, p.copied));
             metrics.add("h2d_device_us", (int64_t)(ms * 1000));
-        }
-        if (sg.tl) {
-            cudaEvent_t dec1 = nullptr;
-            CUDA_OK(cudaEventCreate(&dec1));
-            CUDA_OK(cudaEventRecord(dec1, t.ctx.stream));
-            CUDA_OK(cudaEventSynchronize(dec1));
-            TimelineRow r{0, 0, 0, 0, p.rows};
-            if (p.copy_begin && p.copied) {
-                cudaEventElapsedTime(&r.copy0, tl_base, p.copy_begin);
-                cudaEventElapsedTime(&r.copy1, tl_base, p.copied);
-            }
-            cudaEventElapsedTime(&r.dec0, tl_base, sg.dec0);
-            cudaEventElapsedTime(&r.dec1, tl_base, dec1);
-            timeline.push_back(r);
-            cudaEventDestroy(sg.dec0);
-            cudaEventDestroy(dec1);
-            sg.dec0 = nullptr;
         }
         metrics.add("output_rows", b->num_rows);
         return b;
@@ -1857,7 +1729,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
             Prepared* p;
             ~R() { op->release(*p); }
         } r{this, f->sg.ready.get()};
-        if (f->sg.dec0) cudaEventDestroy(f->sg.dec0);
         if (f->sg.has_jobs) {
             int32_t st = 0;
             CUDA_OK(cudaMemcpy(&st, f->sg.status->ptr, 4, cudaMemcpyDeviceToHost));   // the batch is complete: plain copy, no stream involved
@@ -1866,7 +1737,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
     }
     void retire_fused(Task& t) {
         while (!inflight.empty()) retire_one(t, true);
-        if (!lanes.empty() && !use_lanes) fold_lanes(t);
+        fold_lanes(t);
     }
     void restart(Task& t) override {
         retire_fused(t);
@@ -1874,7 +1745,6 @@ struct ParquetScanExec : Operator, FusedScanSource {
         cur.reset();
         file_pos = 0;
         rg_pos = 0;
-        batches_planned = 0;
         producer_started = producer_done = stop_producer = false;
         producer_err.clear();
         for (auto& kv : metrics.values)
@@ -1883,12 +1753,12 @@ struct ParquetScanExec : Operator, FusedScanSource {
     }
     static bool fused_type_ok(const DType& t) { return t.id == T_INT32 || t.id == T_DATE32 || t.id == T_INT64; }
     bool can_fuse(const FusedAggSpec& spec) const override {
-        if (use_lanes || getenv("AURON_DISABLE_FUSED_SCAN_AGG")) return false;
+        if (getenv("AURON_DISABLE_FUSED_SCAN_AGG")) return false;
         auto col_ok = [&](int c) { return c >= 0 && c < (int)projection.size() && !is_part_col(projection[c]) && fused_type_ok(table_schema.fields[projection[c]].type); };
         if (!col_ok(spec.key_col)) return false;
         // One predicate COLUMN (any number of conjuncts on it: they fold into one interval).  The kernels loop over predicate columns, but
         // that loop has no GPU parity test yet; until it has one, conjunctions over several columns run operator by operator.
-        if (spec.pred_cols.size() > 1 && !getenv("AURON_FUSED_MULTI_PREDICATE")) return false;
+        if (spec.pred_cols.size() > 1) return false;
         for (int c : spec.pred_cols)
             if (!col_ok(c)) return false;
         for (auto& a : spec.accs)
@@ -1973,7 +1843,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
         }
         // key range of this batch from the column-chunk statistics; the table is widened to the union
         const ColState& kcs = p.cols[(size_t)spec.key_col];
-        if (!kcs.stat_ok || getenv("AURON_SCAN_NO_STATS")) return false;
+        if (!kcs.stat_ok) return false;
         long long bmin = kcs.stat_min, bmax = kcs.stat_max;   // min > max: every key of the batch is NULL
         long long umin = bmin, umax = bmax;
         if (st.table && st.has_range) {
@@ -1992,7 +1862,8 @@ struct ParquetScanExec : Operator, FusedScanSource {
 
         const int n_tiles = (int)((n_rows + FZ_TILE - 1) / FZ_TILE);
         struct Phys {
-            Buf dpages, ddicts, seg_base, segs, first_seg, valid;
+            ColDescriptors descr;
+            Buf seg_base, segs, first_seg, valid;
         };
         std::vector<Phys> ph(used.size());
         std::vector<FzScoutCol> scout;
@@ -2001,10 +1872,7 @@ struct ParquetScanExec : Operator, FusedScanSource {
             ColState& cs = p.cols[(size_t)used[u]];
             const int max_def = cs.el.repetition == 1 ? 1 : 0;
             Phys& x = ph[u];
-            x.dpages = to_device(wc, cs.pages.data(), cs.pages.size() * sizeof(PqPage));
-            x.ddicts = to_device(wc, cs.dicts.empty() ? (const void*)"" : (const void*)cs.dicts.data(), cs.dicts.size() * sizeof(PqDict));
-            if (cs.has_v1_inline) pq_fix_v1_pages(wc, P<PqPage>(x.dpages), (int)cs.pages.size(), decomp_results);
-            if (cs.has_delta) pq_delta_to_plain(wc, P<PqPage>(x.dpages), (int)cs.pages.size(), unc_scratch_ptr, cs.el.type == pq::PT_INT32 ? 4 : 8, status_ptr);
+            x.descr = upload_descriptors(wc, cs);
             std::vector<int32_t> sb(cs.pages.size() + 1, 0);
             for (size_t i = 0; i < cs.pages.size(); i++) {
                 const int64_t r0 = cs.pages[i].row_start, n = cs.pages[i].num_values;
@@ -2015,8 +1883,8 @@ struct ParquetScanExec : Operator, FusedScanSource {
             x.first_seg = dalloc_zero(wc, (size_t)n_tiles * 4);
             if (max_def > 0) x.valid = dalloc_zero(wc, (size_t)n_tiles * (FZ_TILE / 8));
             FzScoutCol sc;
-            sc.pages = P<PqPage>(x.dpages);
-            sc.dicts = P<PqDict>(x.ddicts);
+            sc.pages = P<PqPage>(x.descr.pages);
+            sc.dicts = P<PqDict>(x.descr.dicts);
             sc.n_pages = (int32_t)cs.pages.size();
             sc.max_def = max_def;
             sc.seg_base = P<int32_t>(x.seg_base);
@@ -2037,8 +1905,8 @@ struct ParquetScanExec : Operator, FusedScanSource {
             AURON_CHECK(L.ncols < FZ_MAX_COLS, "too many columns in the fused scan");
             const Phys& x = ph[(size_t)phys_of(c)];
             FzColumn& C = L.col[L.ncols];
-            C.pages = P<PqPage>(x.dpages);
-            C.dicts = P<PqDict>(x.ddicts);
+            C.pages = P<PqPage>(x.descr.pages);
+            C.dicts = P<PqDict>(x.descr.dicts);
             C.segs = P<FzSeg>(x.segs);
             C.first_seg = P<int32_t>(x.first_seg);
             C.valid = P<uint32_t>(x.valid);
@@ -2148,9 +2016,9 @@ struct ParquetScanExec : Operator, FusedScanSource {
         // holds (count << shift) | sum(x - min) for the batch: sum(x - min) < rows * 2^bits needs bits + ceil(log2 rows) bits, the
         // count the rest.  min / max come from the chunk statistics; a value outside them raises `oor` like a key would.
         if (L.nacc == 2 && L.acc[0].kind == ACC_SUM_I64 && L.acc[1].kind == ACC_COUNT && L.acc[0].col >= 0 && L.acc[0].col == L.acc[1].col &&
-            L.acc[0].col != L.key_col && !L.acc[0].direct_valid && !L.acc[1].direct_valid && !getenv("AURON_FUSED_NO_PACK")) {
+            L.acc[0].col != L.key_col && !L.acc[0].direct_valid && !L.acc[1].direct_valid) {
             const ColState& vcs = p.cols[(size_t)spec.accs[0].col];
-            if (vcs.stat_ok && vcs.stat_min <= vcs.stat_max && !getenv("AURON_SCAN_NO_STATS")) {
+            if (vcs.stat_ok && vcs.stat_min <= vcs.stat_max) {
                 int bits = 1, rbits = 1;
                 while (bits < 40 && (vcs.stat_max - vcs.stat_min) >= (1ll << bits)) bits++;
                 while ((1ll << rbits) <= n_rows) rbits++;
@@ -2193,7 +2061,6 @@ OperatorPtr make_parquet_scan(Task& t, const uint8_t* node, size_t n) {
     op->host_threads = std::max(1u, std::min(32u, usable_cpus()));
     if (const char* e = getenv("AURON_SCAN_THREADS")) op->host_threads = (unsigned)std::max(1, atoi(e));
     if (const char* e = getenv("AURON_SCAN_PREFETCH_DEPTH")) op->prefetch_depth = atoi(e);
-    if (getenv("AURON_SCAN_NO_PREFETCH")) op->prefetch_depth = 0;
     PbReader r(node, n);
     uint32_t f, w;
     std::vector<std::vector<uint8_t>> prune_exprs;
@@ -2285,7 +2152,7 @@ OperatorPtr make_parquet_scan(Task& t, const uint8_t* node, size_t n) {
         } else r.skip(w);
     }
     // row-group pruning is an optimisation: a predicate this engine cannot fold into per-column intervals prunes nothing
-    if (!prune_exprs.empty() && !getenv("AURON_SCAN_NO_PRUNING")) {
+    if (!prune_exprs.empty()) {
         try {
             std::vector<ExprPtr> es;
             for (auto& b : prune_exprs) es.push_back(decode_expr(b.data(), b.size()));
